@@ -3,7 +3,7 @@
 data-parallel TorchJob at N worker-replica GPUs, with the allreduce's achieved bus bandwidth against
 the NVLink roofline, next to the reference-style gloo/CPU torchjob on the box's host cores.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|nccl]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|nccl] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
       --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -14,7 +14,10 @@ cast/scale/allreduce kernels (through torch_on_k8s_b200's DDP comm hook), + SGD 
 Timing: CUDA events, barrier + synchronize on both sides, MAX over ranks; rank 0 prints ONE JSON
 line.  `value` has inputs resident in HBM; `e2e` copies every step's batch from pinned host memory
 and reads the loss back.  The step's working set (GBs of activations) is far larger than the
-126 MB L2, so no explicit L2 flush is needed between iterations (stated in config.l2).
+50 MB L2 of an H100, so no explicit L2 flush is needed between iterations (stated in config.l2).
+`--dump-outputs DIR` writes what the last timed step computed (loss, and a fixed sample of the
+averaged gradients and updated parameters) as DIR/*.npy, so that two builds can be compared: with
+the same arguments, runs of one build write the same outputs.
 """
 from __future__ import annotations
 
@@ -33,7 +36,9 @@ if ROOT not in sys.path:
 
 METRIC = "resnet50_ddp_images_per_sec"
 UNIT = "images/s"
-NVLINK_PEAK_GBS = 900.0  # nominal per direction per GPU (BASELINE.md §2 fixes this denominator)
+NVLINK_PEAK_GBS = 450.0  # H100 SXM NVLink 4, nominal per direction per GPU (BASELINE.md §2)
+HBM_PEAK_GBS = 3350.0    # H100 SXM HBM3, data sheet
+DUMP_SAMPLE = 1 << 21    # elements of each flattened array --dump-outputs writes (seeded sample)
 
 
 def measured_peaks():
@@ -41,7 +46,7 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:  # noqa: BLE001
-        return {"hbm_gbs": 6650.0}, "fallback"
+        return {"hbm_gbs": HBM_PEAK_GBS}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -109,7 +114,7 @@ def workload_config(batch: int, world: int) -> dict:
                         "into 28.3/22.9 MB; 51.1 MB of gradient/step/replica), SGD momentum 0.9, "
                         "channels_last; 1 master + %d workers" % (batch, world - 1),
             "global_batch": batch * world, "parallelism": "dp%d" % world,
-            "l2": "step working set (GBs of activations) is larger than the 126 MB L2; no explicit "
+            "l2": "step working set (GBs of activations) is larger than the 50 MB L2; no explicit "
                   "flush",
             "allreduce_bytes_per_step": RESNET50_BF16_BYTES_PER_STEP}
 
@@ -198,6 +203,25 @@ def parity_check(rep, sizes, world, zero_copy, stream):
                        "bit for bit on every replica before timing"}
 
 
+def dump_outputs(out_dir, model, loss):
+    """What the last timed step handed back: its loss, and a seeded sample (same indices in every
+    run) of the gradients averaged by the bucket exchange and of the parameters SGD updated, in
+    model.parameters() order, as float32 .npy files."""
+    import numpy as np
+    import torch
+    params = list(model.parameters())
+    flat_p = torch.cat([p.detach().reshape(-1).float() for p in params])
+    flat_g = torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).detach()
+                        .reshape(-1).float() for p in params])
+    n = min(DUMP_SAMPLE, flat_p.numel())
+    idx = np.sort(np.random.default_rng(0).choice(flat_p.numel(), n, replace=False))
+    idx = torch.from_numpy(idx).to(flat_p.device)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    np.save(os.path.join(out_dir, "grads_sample.npy"), flat_g[idx].cpu().numpy())
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat_p[idx].cpu().numpy())
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -227,7 +251,11 @@ def run_ours(args):
 
     rep = init_replica(device=local)
     dev = rep.device
-    torch.backends.cudnn.benchmark = True
+    # cuDNN's autotuner times candidate kernels in each new process and may settle on different
+    # convolution algorithms from one run to the next, which changes the step's rounding; with
+    # heuristic selection and deterministic algorithms, the same arguments give the same outputs
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True
     B = args.batch
     nccl_only = args.impl == "nccl"
 
@@ -361,9 +389,15 @@ def run_ours(args):
     if rank == 0:
         sampler.start()
     launches0 = rep.comm.launches()
-    ms_dev = timed(lambda i: step(dev_x, dev_y), args.steps)
+    last = {}
+
+    def timed_step(i):
+        last["loss"] = step(dev_x, dev_y)
+    ms_dev = timed(timed_step, args.steps)
     launches = rep.comm.launches() - launches0
     ev = hook.drain_events()
+    if args.dump_outputs and rank == 0:   # replicas hold identical parameters and gradients
+        dump_outputs(args.dump_outputs, ddp.module, last["loss"])
 
     # ---- end-to-end leg: host batch -> device every step, loss read back every step --------------
     def e2e_step(i):
@@ -394,46 +428,26 @@ def run_ours(args):
     ar_ms_max = float(stats[1].item())
     wait_ms_max = float(stats[2].item())
     kernel_name = rep.comm.last_algo()
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            tr = json.load(f).get(kernel_name, {})
-        per = [tr.get(str(sz)) for sz in sizes]
-        if per and all(v is not None for v in per):
-            traffic = sum(per) / len(per)
-    except Exception:  # noqa: BLE001
-        traffic = None
     if world == 1:
         # fused scale/cast only: S_in + S_out against HBM
         achieved = (2.0 * bucket_bytes) / (ar_ms_max * 1e-3) / 1e9 if ar_ms_max > 0 else 0.0
         roof = {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": achieved / peaks["hbm_gbs"], "traffic": traffic,
+                "frac": achieved / peaks["hbm_gbs"],
                 "kernel": "tok::%s_kernel<bf16>" % kernel_name,
                 "algorithmic_bytes_per_launch": 2.0 * bucket_bytes / n_launch,
                 "avg_launch_us": ar_ms_max * 1e3 / n_launch, "peak_source": peak_kind + " hbm_gbs",
-                "traffic_source": "dram__bytes_read.sum + dram__bytes_write.sum per launch, ncu "
-                                  "--set full at these bucket sizes (profiles/traffic.json)",
                 "note": "world=1 degenerates to the fused scale/cast: bytes = S_in + S_out; one "
-                        "launch between two CUDA events, launch latency included.  traffic is about "
-                        "S_in alone: the in-place result stays in the 126 MB L2 (written back after "
-                        "the kernel), and the kernel is latency-bound at this size (ncu: DRAM at "
-                        "~30 % of peak for ~10 us) — ATen's own mul_ takes the same 12.3 us "
-                        "back to back on the 28 MB bucket (profiles/r02_local_bench_n1.json)"}
+                        "launch between two CUDA events, launch latency included"}
     else:
         algbw = wire_bytes / (ar_ms_max * 1e-3) / 1e9 if ar_ms_max > 0 else 0.0
         busbw = algbw * 2.0 * (world - 1) / world
         roof = {"bound": "nvlink", "achieved": busbw, "peak": NVLINK_PEAK_GBS, "unit": "GB/s",
-                "frac": busbw / NVLINK_PEAK_GBS, "traffic": traffic,
+                "frac": busbw / NVLINK_PEAK_GBS,
                 "kernel": "tok::%s_kernel<bf16>" % kernel_name,
                 "algbw_gbs": algbw, "algorithmic_bytes_per_launch": wire_bytes / n_launch,
                 "avg_launch_us": ar_ms_max * 1e3 / n_launch,
                 "arrival_wait_us": wait_ms_max * 1e3 / n_launch,
-                "peak_source": "nominal NVLink5 900 GB/s per direction (BASELINE.md §2); measured "
-                               "peer copy on this pool is 770 GB/s",
-                "traffic_note": "ncu cannot replay a kernel that waits for peer replicas' kernels, so "
-                                "there is no dram__bytes capture for the cross-GPU kernels; the "
-                                "zero-copy exchange makes no staging pass by construction (reads of "
-                                "the bucket by the switch / peers + one write of the result)",
+                "peak_source": "nominal NVLink 4 450 GB/s per direction (H100 SXM, BASELINE.md §2)",
                 "note": "busbw = S/t * 2(N-1)/N over the exchange kernels inside the timed steps, "
                         "concurrent with backward; the wait for the slowest replica is the 1-warp "
                         "arrival kernel in front (arrival_wait_us), not part of t; NVLS may exceed 1.0"}
@@ -498,7 +512,7 @@ def run_ours(args):
         iso["kernel"] = rep.comm.last_algo()
         iso["zero_copy"] = bool(zero_copy)
         iso["note"] = ("the step's buckets exchanged back to back on an otherwise idle GPU (arrival "
-                       "kernels included), inputs rotated over >126 MB so they are not L2 resident")
+                       "kernels included), inputs rotated over >160 MiB so they are not L2 resident")
         del sets
 
     # ---- stock DDP + NCCL on the same box, same process, right after (N > 1) -----------------------
@@ -571,7 +585,13 @@ def main():
     ap.add_argument("--no-nccl", action="store_true", help="skip the stock DDP+NCCL comparison leg")
     ap.add_argument("--cpu-steps", type=int, default=3)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="our arm: write the last timed step's loss and a fixed sample of its "
+                         "averaged gradients and updated parameters to DIR/*.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs records our arm's timed step; it is not available with --impl %s"
+                 % args.impl)
     if args.impl == "reference":
         return run_reference(args)
     return run_ours(args)

@@ -1,5 +1,5 @@
 /*
- * tok8s.h — C ABI of libtok8s, the B200-native drop-in for the data-parallel hot path of
+ * tok8s.h — C ABI of libtok8s, the H100-native drop-in for the data-parallel hot path of
  * hliangzhao/torch-on-k8s (per-step DDP gradient-bucket allreduce behind the TorchJob surface).
  *
  * The reference is a pure-Go operator built with CGO_ENABLED=0 (reference Dockerfile:19); it has
@@ -28,7 +28,7 @@ extern "C" {
 #endif
 
 #define TOK_ABI_VERSION 2
-#define TOK_MAX_WORLD 8 /* one 8xB200 box: one replica per GPU */
+#define TOK_MAX_WORLD 8 /* one 8-GPU H100 box: one replica per GPU */
 
 /* ---- error codes ------------------------------------------------------------------------- */
 enum {

@@ -11,7 +11,8 @@ Fixtures
       native-dtype bf16 all_reduce of bf16(x)/N ["bf16_native"] (informational: gloo sums in bf16).
   sampler.json                    DistributedSampler indices for several (len, world, epoch, seed).
   mlp_torchjob_n2/                BASELINE config 0: 2-layer MLP, 1 master + 1 worker, gloo: losses,
-      per-bucket pre/post tensors, argmax, final weights of rank 0 and 1.
+      per-bucket pre/post tensors, argmax, final weights of rank 0 and 1 (the flat tensors are a
+      seeded sample of MLP_SAMPLE elements, the same indices in every array, to keep each file small).
 """
 from __future__ import annotations
 
@@ -30,6 +31,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 COUNT = 4099
 SEED = 4242
+MLP_SAMPLE = 32768
 
 
 def _rank(rank, world, port, q):
@@ -127,12 +129,29 @@ def make_sampler():
         json.dump(out, f)
 
 
+def sample_mlp_dump(d):
+    """Keeps the same seeded MLP_SAMPLE indices of every flat per-parameter-element array (bucket
+    pre/post tensors, final weights) of each rank's dump; the checks on them are element-wise."""
+    for name in sorted(os.listdir(d)):
+        if not name.endswith(".npz"):
+            continue
+        with np.load(os.path.join(d, name)) as z:
+            arrs = {k: z[k] for k in z.files}
+        n = arrs["final_flat"].shape[0]
+        if n <= MLP_SAMPLE:
+            continue
+        idx = np.sort(np.random.default_rng(SEED).choice(n, MLP_SAMPLE, replace=False))
+        arrs = {k: (v[idx] if v.ndim == 1 and v.shape[0] == n else v) for k, v in arrs.items()}
+        np.savez_compressed(os.path.join(d, name), **arrs)
+
+
 def make_mlp():
     from oracle import gloo_torchjob
     d = os.path.join(HERE, "mlp_torchjob_n2")
     shutil.rmtree(d, ignore_errors=True)
     res = gloo_torchjob.run("mlp", world=2, steps=2, warmup=0, batch=64, threads=1, dtype="f32",
                             dump=d, job="golden-mlp")
+    sample_mlp_dump(d)
     with open(os.path.join(d, "run.json"), "w") as f:
         json.dump(dict(losses=res["losses"], steps=2, batch=64, lr=0.01, world=2), f)
 

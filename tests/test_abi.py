@@ -29,7 +29,7 @@ def test_python_prototypes_match_header(tok_lib):
 
 
 def test_version_and_error_plumbing(tok_lib):
-    assert b"sm_100a" in tok_lib.tok_version()
+    assert b"sm_90a" in tok_lib.tok_version()
     from torch_on_k8s_b200 import _ffi
     h = ctypes.c_void_p()
     rc = tok_lib.tok_comm_create(b"j", 3, 2, 8, 0, b"/tmp/x", ctypes.byref(h))

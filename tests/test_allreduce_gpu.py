@@ -49,6 +49,20 @@ def test_world1_local_kernel(tok_lib):
     assert_all_exact(res, len(cases), 1)
 
 
+def test_rendezvous_under_a_long_directory(tok_lib, n_gpus, tmp_path, monkeypatch):
+    """A rendezvous file whose socket path does not fit a unix socket address (108 bytes) still
+    forms the group: the socket moves to the abstract namespace under a name derived from the path."""
+    import tempfile
+    deep = tmp_path / ("d" * 100) / ("e" * 40)
+    deep.mkdir(parents=True)
+    monkeypatch.setattr(tempfile, "tempdir", str(deep))
+    devs, env = devices_for(2, n_gpus)
+    cases = [dict(count=4097, **{"in": "bf16", "wire": "bf16", "out": "bf16"}, algo=2, seed=31,
+                  scale=0.5)]
+    res = harness.launch(2, cases, devices=devs, mode="thread", timeout=120, env=env)
+    assert_all_exact(res, len(cases), 2)
+
+
 def test_world1_identity_bucket_is_elided(tok_lib):
     """in == out, one dtype, scale 1 at world 1 is already the answer: no launch, no HBM pass — unless
     the caller insists (TOK_FLAG_NO_ELIDE), in which case the kernel runs and changes nothing."""

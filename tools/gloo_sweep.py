@@ -1,6 +1,7 @@
 """CPU column of BASELINE config 4: standalone torch.distributed gloo all_reduce sweep (the
 reference-style backend), N local processes wired per SetClusterSpec, busbw = S/t * 2(N-1)/N.
 Runs anywhere (no GPU).  Not part of the product."""
+import argparse
 import json
 import multiprocessing as mp
 import os
@@ -42,6 +43,10 @@ def _rank(rank, world, port, sizes, threads, q):
 
 
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", help="also write the whole sweep to this JSON file (the rows are "
+                                  "printed as JSON lines either way)")
+    args = ap.parse_args()
     from oracle.gloo_torchjob import effective_cores, free_port
     sizes = [4096 << (2 * k) for k in range(0, 8)]   # 4 KiB .. 64 MiB
     out = dict(cores=effective_cores(), when=time.time(), rows=[])
@@ -56,10 +61,10 @@ def main():
         [p.join() for p in ps]
         for r in out["rows"][-len(sizes) * 2:]:
             print(json.dumps({k: (round(v, 3) if isinstance(v, float) else v) for k, v in r.items()}), flush=True)
-    path = os.path.join(ROOT, "profiles", "r01_gloo_sweep_cpu_%dcores.json" % out["cores"])
-    with open(path, "w") as f:
-        json.dump(out, f, indent=1)
-    print("wrote", path)
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump(out, f, indent=1)
+        print("wrote", args.out)
 
 
 if __name__ == "__main__":

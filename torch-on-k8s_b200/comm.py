@@ -1,7 +1,7 @@
 """Replica communicator — Python face of tok_comm_* / tok_allreduce_bucket (include/tok8s.h).
 
 One Communicator per worker replica (= one process bound to one GPU).  PyTorch is used only for
-device memory and streams; the reduction itself is libtok8s' sm_100a kernels.
+device memory and streams; the reduction itself is libtok8s' sm_90a kernels.
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 """Single-box TorchJob controller: the reference operator's reconcile loop for the data-parallel
-path, with "pod" = OS process bound to one GPU of the 8xB200 box.
+path, with "pod" = OS process bound to one GPU of the 8-GPU H100 box.
 
   reference                                            here
   -------------------------------------------------    ------------------------------------------------

@@ -1,5 +1,5 @@
 // allreduce.cu — the data-parallel hot path: per-step DDP gradient-bucket allreduce across the
-// job's replicas, fused with the bucket cast/scale, hand-written for sm_100a.
+// job's replicas, fused with the bucket cast/scale, hand-written for sm_90a (H100).
 //
 // Replaces (reference side, third-party): DDP default comm hook `tensor.div_(N)` + `all_reduce`
 // (torch/distributed/algorithms/ddp_comm_hooks/default_hooks.py:18-33), the compress hooks' cast +

@@ -274,6 +274,7 @@ struct Star {
   int listen_fd = -1;
   std::vector<int> conn;  // root: conn[rank] for rank != 0 ; member: conn[0] = link to root
   std::string path;
+  bool abstract_sock = false;  // the socket lives in the abstract namespace: no file to unlink
   double deadline = 0;
 
   ~Star() { close_all(); }
@@ -286,7 +287,7 @@ struct Star {
     if (listen_fd >= 0) {
       close(listen_fd);
       listen_fd = -1;
-      unlink(path.c_str());
+      if (!abstract_sock) unlink(path.c_str());
     }
   }
   // Collective AND of a per-member status, returned to everyone.
@@ -336,7 +337,7 @@ struct tok_comm {
   uint64_t epoch = 0;
   CUdevice cu_dev = 0;
   char bus_id[32] = {0};
-  int sm_count = 148;
+  int sm_count = 132;
   int mc_supported = 0;
 
   size_t gran = 0;
@@ -527,10 +528,23 @@ int exchange(tok_comm* c) {
   struct sockaddr_un addr;
   memset(&addr, 0, sizeof(addr));
   addr.sun_family = AF_UNIX;
-  if (star.path.size() >= sizeof(addr.sun_path))
-    return fail(TOK_ERR_INVALID, "rendezvous path too long (%zu >= %zu): %s", star.path.size(),
-                sizeof(addr.sun_path), star.path.c_str());
-  strcpy(addr.sun_path, star.path.c_str());
+  // A socket path must fit sun_path (108 bytes); a rendezvous file under a long directory (a
+  // deep TMPDIR, say) gets a socket in the abstract namespace instead, named by a hash of its path
+  // so that every replica of the group derives the same name.  An abstract name has no filesystem
+  // permissions: any process in the same network namespace could bind it first.  The group still
+  // checks every Hello (magic, ABI, job, epoch, rank) and maps only heaps whose identity token
+  // matches, so a squatter makes the rendezvous fail rather than join; a short rendezvous path in a
+  // private directory avoids the abstract namespace altogether.
+  star.abstract_sock = star.path.size() >= sizeof(addr.sun_path);
+  const bool abstract_sock = star.abstract_sock;
+  if (abstract_sock) {
+    uint64_t h = 1469598103934665603ull;  // FNV-1a
+    for (unsigned char ch : star.path) h = (h ^ ch) * 1099511628211ull;
+    snprintf(addr.sun_path + 1, sizeof(addr.sun_path) - 1, "tok8s-%016llx",
+             static_cast<unsigned long long>(h));
+  } else {
+    strcpy(addr.sun_path, star.path.c_str());
+  }
 
   Hello me;
   memset(&me, 0, sizeof(me));
@@ -571,7 +585,7 @@ int exchange(tok_comm* c) {
       close(my_fd);
       return fail(TOK_ERR_RENDEZVOUS, "socket(): %s", strerror(errno));
     }
-    unlink(star.path.c_str());
+    if (!abstract_sock) unlink(star.path.c_str());
     if (bind(star.listen_fd, reinterpret_cast<struct sockaddr*>(&addr), sizeof(addr)) != 0 ||
         listen(star.listen_fd, kMaxWorld) != 0) {
       close(my_fd);
@@ -894,9 +908,8 @@ int create_impl(const char* job_id, int rank, int world, int max_world, int devi
   // NCCL's watchdog default is 600 s; replicas legitimately skew by tens of seconds (first-iteration
   // cuDNN autotune, evaluation or a checkpoint on rank 0)
   c->barrier_timeout_ns = env_size("TOK_BARRIER_TIMEOUT_MS", 600000) * 1000000ull;
-  // measured (profiles/r02_local_bench_n1.json): the cp.async.bulk ring beats the LDG.128 wave at
-  // every size from 4 MB to 1 GiB (12.4 vs 14.5 us at the 28 MB DDP bucket, 0.97 vs 0.71-0.90 of the
-  // measured HBM peak at 1 GiB)
+  // the cp.async.bulk ring is the default for same-dtype buckets from 1 MiB (tools/local_bench.py
+  // compares it with the LDG.128 wave; DESIGN.md §6 has the H100 numbers)
   c->local_tma = static_cast<int>(env_size("TOK_LOCAL_TMA", 1));
   c->nvls_unroll = env_size("TOK_NVLS_UNROLL", 8) == 16 ? 16 : 8;
   c->rdzv_timeout_s = static_cast<double>(env_size("TOK_RDZV_TIMEOUT_S", 120));
@@ -924,7 +937,8 @@ int create_impl(const char* job_id, int rank, int world, int max_world, int devi
   return TOK_OK;
 }
 
-// Algorithm selector.  Thresholds come from the measured sweeps on 2/4/8 B200 (profiles/): one-shot
+// Algorithm selector.  The thresholds were tuned on an 8-GPU NVSwitch system and have not been
+// re-measured on H100 (NVLink 4, 450 GB/s per direction); the shape of the rule holds: one-shot
 // moves (N-1)*S per GPU but needs a single barrier, so it wins while the bucket is latency-bound —
 // the smaller the group, the longer; NVLS wins as soon as there are >= 3 replicas and the bucket is
 // past the one-shot range; at N == 2 the in-switch reduction saves nothing and two-shot is faster.
@@ -949,8 +963,8 @@ int pick_algo(const tok_comm* c, size_t wire_bytes) {
   }
   const size_t slot = c->cap_bytes / kMaxWorld;
   if (wire_bytes <= one_shot_limit(c) && wire_bytes <= slot) return TOK_ALGO_ONE_SHOT;
-  // staged path: with 3-4 replicas the in-switch reduction stops paying off past ~12 MiB (measured:
-  // two-shot 385 vs NVLS 335 GB/s busbw at 16 MiB, N=4); zero-copy buckets re-promote to NVLS
+  // staged path: with 3-4 replicas the in-switch reduction stops paying off past ~12 MiB (two-shot
+  // beat NVLS at 16 MiB, N=4, in the tuning sweeps); zero-copy buckets re-promote to NVLS
   const bool nvls_ok = c->mc_va && c->world >= 3 && wire_bytes >= c->nvls_min;
   if (nvls_ok && (c->world >= 5 || wire_bytes < (12u << 20))) return TOK_ALGO_NVLS;
   return TOK_ALGO_TWO_SHOT;
@@ -965,7 +979,7 @@ extern "C" {
 
 const char* tok_last_error(void) { return tok::last_error_cstr(); }
 
-const char* tok_version(void) { return "libtok8s 0.2 (sm_100a, abi 2)"; }
+const char* tok_version(void) { return "libtok8s 0.2 (sm_90a, abi 2)"; }
 
 void tok_free(void* p) { free(p); }
 
@@ -1295,8 +1309,8 @@ int plan_bucket(const tok_comm* c, const void* in, const void* out, size_t count
   // in place, in its own dtype, in whole 16-byte packs -> peers read / multicast it directly.
   const bool pool_ok = c->zero_copy && !(flags & TOK_FLAG_NO_ZERO_COPY) && in == out && same_dt &&
                        in_pool(c, in, count * isz) && (count * wsz) % 16 == 0;
-  // a pool bucket leaves the one-shot range earlier: its exchange needs no staging pass (measured at
-  // N=2, profiles/r02_sweep_n2.json: in place 30.9 vs one-shot 30.0 us at 8 MiB, 43.6 vs 47.0 at 16)
+  // a pool bucket leaves the one-shot range earlier: its exchange needs no staging pass (in the N=2
+  // tuning sweeps the in-place exchange caught up with one-shot at 8 MiB and beat it at 16 MiB)
   if (!forced && algo == TOK_ALGO_ONE_SHOT && pool_ok && c->world == 2 && count * wsz >= (8u << 20))
     algo = TOK_ALGO_TWO_SHOT;
   bool inplace = pool_ok && (algo == TOK_ALGO_TWO_SHOT || algo == TOK_ALGO_NVLS);
@@ -1308,9 +1322,8 @@ int plan_bucket(const tok_comm* c, const void* in, const void* out, size_t count
     const bool post = (flags & TOK_FLAG_SCALE_POST) != 0;
     const bool nvls_exact = (post || is_pow2_scale(scale)) && (wire_dtype != TOK_F16 || post);
     // (pick_algo's rule stands for pool buckets too: with 3-4 replicas the in-switch reduction stops
-    // paying off past ~12 MiB — measured in place at N=4 on the 22.9 / 28.3 MB DDP buckets: P2P
-    // reduce+push 83.0 us vs NVLS 95.7 us, profiles/r02_zc_tune_n4.json; with >= 5 replicas NVLS wins:
-    // 81 vs 98 us at N=8, profiles/r02_zc_tune_n8.json)
+    // paying off past ~12 MiB — P2P reduce+push beat NVLS in place at N=4 on the 22.9 / 28.3 MB DDP
+    // buckets in the tuning sweeps; with >= 5 replicas NVLS won)
     if (algo == TOK_ALGO_NVLS && !nvls_exact) {
       if (forced)
         inplace = false;  // honour the forced algorithm through the staged kernel
@@ -1434,10 +1447,9 @@ int tok_allreduce_bucket(tok_comm_t* c, const void* in, void* out, size_t count,
       size_t cap_ctas = c->max_ctas;
       if (inplace) {
         // In-place NVLS saturates the NVSwitch reduction path with few requesters: in the isolated
-        // sweeps (profiles/r01_sweep_n{4,8}_zero_copy_cta_tuning.json) 16 CTAs beat 64 from 32 MiB
-        // up at N=8 (91 vs 112 us at 32 MiB, 160 vs 184 at 64 MiB).  Below that the evidence is
-        // within run-to-run noise, and the ResNet-50 buckets (22.9 / 28.3 MB) measured best with 64
-        // CTAs inside bench.py (77 us/bucket vs 87 with 16-32 CTAs), so 64 stays the default there.
+        // tuning sweeps 16 CTAs beat 64 from 32 MiB up at N=8.  Below that the difference was within
+        // run-to-run noise, and the ResNet-50 buckets (22.9 / 28.3 MB) did best with 64 CTAs inside
+        // bench.py, so 64 stays the default there.  (Not re-measured on H100.)
         if (c->zc_ctas)
           cap_ctas = c->zc_ctas;
         else if (algo == kAlgoNvlsInplace && bytes >= (32u << 20))

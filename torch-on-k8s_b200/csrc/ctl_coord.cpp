@@ -1,5 +1,5 @@
 // ctl_coord.cpp — job coordinator: tenant queues + plugin pipeline of pkg/coordinator, re-targeted
-// from ResourceQuota objects to the GPU slots of one 8xB200 box.
+// from ResourceQuota objects to the GPU slots of one 8-GPU H100 box.
 //
 //   schedule cycle      pkg/coordinator/core/coordinator.go:310-366
 //   queue selection     RR  core/policy.go:31-76 ; WRR core/policy.go:80-230 (default here: the

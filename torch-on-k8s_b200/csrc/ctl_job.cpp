@@ -92,7 +92,7 @@ std::string job_namespace(const tok_job* j) {
 }
 
 // GPU slots one replica of this task type occupies on the box.  The reference sums container
-// resource requests (pkg/utils/resources/resources.go:56-72); on one 8xB200 box the only resource is
+// resource requests (pkg/utils/resources/resources.go:56-72); on one 8-GPU H100 box the only resource is
 // nvidia.com/gpu (apis/train/v1alpha1/constants.go:28) and every training replica is bound to exactly
 // one GPU unless the template asks for more.  AIMaster defaults to zero (it does not train).
 int64_t replica_slots(const std::string& task_type, const json::Value& ts) {

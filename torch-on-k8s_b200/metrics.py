@@ -39,7 +39,7 @@ class Metrics:
         # coordinator (core/metrics.go:25-28)
         self.queue_pending = Gauge("torch_on_k8s_tenant_queue_jobs_pending_count",
                                    "Counts number of jobs pending in queue", ["queue"], registry=r)
-        # new series for the B200 path
+        # new series for the H100 path
         self.busbw = Gauge("torch_on_k8s_allreduce_busbw_gbps",
                            "Achieved allreduce bus bandwidth of the last step (GB/s)", ["job"], registry=r)
         self.reform_latency = Histogram("torch_on_k8s_reform_latency_seconds",
