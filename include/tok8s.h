@@ -130,10 +130,18 @@ int tok_comm_caps(tok_comm_t* comm, tok_caps_t* caps);
  * same sequence of calls with the same count / dtypes / flags.  Buckets that live in the symmetric
  * pool (below) are exchanged in place without staging: a 1-warp arrival kernel ("my bucket is ready",
  * wait for every peer's, symmetry check) followed by the exchange kernel.  The P2P in-place kernel
- * honours PRE/POST exactly like the staged path (bit-identical to it); the NVSwitch (NVLS) in-place
- * kernel can only scale the sum, so AUTO uses it when that is the same function — POST, or `scale`
- * a power of two (1/N for N = 2, 4, 8) — and never for an f16 PRE bucket (the sum could overflow
- * before it is scaled); otherwise AUTO takes the P2P in-place kernel. */
+ * honours PRE/POST exactly like the staged path (bit-identical to it).  NVSwitch (NVLS) summation
+ * returns the sum in an unspecified order, rounded to the wire dtype, and its in-place kernel can
+ * only scale that sum.  AUTO therefore uses NVLS only where this is the specified function up to
+ * summation order: a PRE bucket in place only with `scale` a power of two (1/N for N = 2, 4, 8) and
+ * never with an f16 wire (the sum could overflow before it is scaled); a POST bucket, staged or in
+ * place, only with an f32 wire or a bf16 wire and a power-of-two `scale` (otherwise the sum is rounded
+ * twice, and an f16 sum can overflow before the scale).  Power-of-two factors are exact except where
+ * the unscaled sum leaves the wire dtype's range or the result is subnormal.  Every other bucket
+ * takes a P2P kernel.  tok_allreduce_algo() answers for the size alone, before this rule.
+ * TOK_ALGO_NVLS passed in `flags` runs NVLS whatever the scale and dtypes, within the NVLS
+ * tolerance; the TOK_ALGO environment variable only replaces AUTO's choice by size, and the rules
+ * above still apply to it. */
 int tok_allreduce_bucket(tok_comm_t* comm, const void* in, void* out, size_t count, int in_dtype,
                          int wire_dtype, int out_dtype, float scale, unsigned flags,
                          void* cuda_stream);

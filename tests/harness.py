@@ -43,9 +43,101 @@ def gen_input(seed: int, rank: int, count: int, dtype: str, pattern: str = "rand
         x = np.full(count, float(rank + 1), dtype=np.float32)
     elif pattern == "wide":  # wide dynamic range: exposes accumulation-order differences
         x = (rs.standard_normal(count) * np.exp(rs.uniform(-12, 12, size=count))).astype(np.float32)
+    elif pattern == "special":  # IEEE edge values (SPECIAL_RECIPES) over a randn background
+        x = rs.standard_normal(count).astype(np.float32)
+        idx, u = special_layout(seed, count)
+        for k, (_, fn) in enumerate(SPECIAL_RECIPES):
+            sel = idx == k
+            if sel.any():
+                x[sel] = fn(rank, u[sel], dtype)
     else:
         raise ValueError(pattern)
     return from_f32(x, dtype)
+
+
+# ---- the "special" pattern ------------------------------------------------------------------------
+# Rank-dependent recipes: fn(rank, u, in_dtype) -> the fp32 value replica `rank` holds (u: a shared,
+# rank-independent uniform in [0.5, 2)).  The value is then rounded to the in dtype like any input.
+# Element i takes recipe i % len(SPECIAL_RECIPES); the length is odd (coprime to the 4- and 8-element
+# packs), so every recipe lands in every lane of a pack and, across counts, in the ragged tail.
+def _f32(bits: int) -> np.float32:
+    return np.array([bits], dtype=np.uint32).view(np.float32)[0]
+
+
+_NZ = np.float32(-0.0)
+_INF = np.float32(np.inf)
+_MAX = {"f32": np.float32(np.finfo(np.float32).max), "bf16": _f32(0x7F7F0000),
+        "f16": np.float32(65504.0)}
+
+
+def _on(ranks, val, other=_NZ):
+    """`val` on the listed ranks, `other` (default -0.0, the identity of the sum) elsewhere."""
+    return lambda r, u, dt: np.float32(val) if r in ranks else (other(u) if callable(other)
+                                                               else np.float32(other))
+
+
+SPECIAL_RECIPES = (
+    ("neg_zero", lambda r, u, dt: _NZ),                              # -0 + -0 = -0
+    ("pos_zero_rank0", _on((0,), 0.0)),                              # +0 + -0 = +0
+    ("x_minus_x", lambda r, u, dt: u if r == 0 else (-u if r == 1 else _NZ)),
+    ("inf_one_rank", _on((1,), np.inf, other=lambda u: u)),
+    ("inf_minus_inf", lambda r, u, dt: _INF if r == 0 else (-_INF if r == 1 else u)),
+    ("nan_one_rank", _on((0,), np.nan, other=lambda u: u)),
+    ("max_finite", lambda r, u, dt: _MAX[dt]),                       # fp32 sum overflows (f32, bf16)
+    # rank order: (2^12 + 2^-12) rounds to 2^12 (a tie, to even), - 2^12 = 0; any other order gives
+    # 2^-12.  Exact in every dtype, so it survives the PRE cast at power-of-two scales.
+    ("order_triple", lambda r, u, dt: np.float32([2.0 ** 12, 2.0 ** -12, -2.0 ** 12][r]) if r < 3
+     else _NZ),
+    ("f32_min_subnormal", lambda r, u, dt: np.float32(2.0 ** -149)),
+    ("f32_max_subnormal", lambda r, u, dt: _f32(0x007FFFFF)),
+    ("f32_min_normal", lambda r, u, dt: np.float32(2.0 ** -126)),     # also bf16's
+    ("bf16_min_subnormal", lambda r, u, dt: np.float32(2.0 ** -133)),
+    ("bf16_max_subnormal", lambda r, u, dt: _f32(0x007F0000)),
+    ("f16_min_subnormal", lambda r, u, dt: np.float32(2.0 ** -24)),
+    ("f16_max_subnormal", lambda r, u, dt: np.float32(1023 * 2.0 ** -24)),
+    ("f16_min_normal", lambda r, u, dt: np.float32(2.0 ** -14)),
+    # just above the smallest normal: a scale below 1 moves them into the subnormal range ...
+    ("into_subnormal", lambda r, u, dt: np.float32((1 + (r + 1) / 16.0) * 2.0 ** -126)),
+    ("into_subnormal_f16", lambda r, u, dt: np.float32((1 + (r + 1) / 16.0) * 2.0 ** -14)),
+    # ... and subnormals that a scale above 1 (2^20) makes normal
+    ("out_of_subnormal", lambda r, u, dt: np.float32((r + 1) * 2.0 ** -130)),
+    ("out_of_subnormal_f16", lambda r, u, dt: np.float32((r + 1) * 2.0 ** -22)),
+    # fp32 values around the overflow threshold of a bf16 / f16 cast
+    ("bf16_ovf_below", _on((0,), _f32(0x7F7F7FFF))),
+    ("bf16_ovf_at", _on((0,), _f32(0x7F7F8000))),
+    ("bf16_ovf_above", _on((0,), _f32(0x7F7F8001))),
+    ("f16_ovf_below", _on((0,), np.nextafter(np.float32(65520.0), np.float32(0.0)))),
+    ("f16_ovf_at", _on((0,), 65520.0)),
+    # sums that land exactly on a rounding tie of a 16-bit cast: down (to even) and up (to even)
+    ("tie_sum_bf16_down", lambda r, u, dt: np.float32([1.0, 2.0 ** -8][r]) if r < 2 else _NZ),
+    ("tie_sum_bf16_up", lambda r, u, dt: np.float32([1 + 2.0 ** -7, 2.0 ** -8][r]) if r < 2 else _NZ),
+    ("tie_sum_f16_down", lambda r, u, dt: np.float32([1.0, 2.0 ** -11][r]) if r < 2 else _NZ),
+    ("tie_sum_f16_up", lambda r, u, dt: np.float32([1 + 2.0 ** -10, 2.0 ** -11][r]) if r < 2 else _NZ),
+    # fp32 inputs that are themselves ties of the wire cast, down on even ranks, up on odd ones
+    ("tie_wire_bf16", lambda r, u, dt: np.float32(1 + (2 * (r % 2) + 1) * 2.0 ** -8)),
+    ("tie_wire_f16", lambda r, u, dt: np.float32(1 + (2 * (r % 2) + 1) * 2.0 ** -11)),
+)
+assert len(SPECIAL_RECIPES) % 2 == 1
+SPECIAL_INDEX = {name: k for k, (name, _) in enumerate(SPECIAL_RECIPES)}
+
+
+def special_scales(world: int):
+    """(scale, post) pairs for the edge-value tests: 1/N, 1/3 both ways, and factors that overflow the
+    wire cast (2^20), make results subnormal (2^-140) or flip signs (-0.5), PRE and POST."""
+    out = [(1.0 / world, False), (1.0 / 3.0, False), (1.0 / 3.0, True)]
+    for s in (2.0 ** -3, 2.0 ** 20, 2.0 ** -140, -0.5):
+        out += [(s, False), (s, True)]
+    return out
+
+
+def special_layout(seed: int, count: int):
+    """(recipe index per element, -1 where the randn background stays; shared u values).  Depends on
+    the seed only, so every replica places the same recipe at the same element."""
+    rs = np.random.RandomState((seed * 7 + 3) % (2 ** 31 - 1))
+    background = rs.random_sample(count) < 0.2
+    idx = np.where(background, -1, np.arange(count) % len(SPECIAL_RECIPES))
+    u = rs.uniform(0.5, 2.0, size=count).astype(np.float32)
+    return idx, u
 
 
 def to_torch(a: np.ndarray, dtype: str, device):
@@ -131,8 +223,24 @@ def run_cases(rank: int, world: int, device: int, path: str, cases: List[dict],
                 continue
             inputs = [gen_input(seed, r, count, din, pattern) for r in range(world)]
             want = allreduce_oracle(inputs, din, dw, dout, scale, post)
+            # guard: the bucket is the middle of count + 2*guard elements whose ends hold GUARD_BYTE
+            guard = case.get("guard", 0)
+            xf = yf = None
             with torch.cuda.stream(stream):
-                if symm:
+                if guard:
+                    alloc = symm_empty if symm else \
+                        (lambda n, dt: torch.empty(n, dtype=dt, device=dev))
+                    xf = _guarded(alloc, count, guard, torch_dtype(din))
+                    x = xf[guard:guard + count]
+                    x.copy_(to_torch(inputs[rank], din, dev))
+                    if symm:
+                        assert comm.in_symmetric_pool(x)
+                    if symm or inplace:
+                        y, yf = x, xf
+                    else:
+                        yf = _guarded(alloc, count, guard, torch_dtype(dout))
+                        y = yf[guard:guard + count]
+                elif symm:
                     if case.get("skew") and rank == world - 1:
                         _extra = symm_empty(count, torch_dtype(din))  # steals x's block
                     x = symm_empty(count, torch_dtype(din))
@@ -164,11 +272,25 @@ def run_cases(rank: int, world: int, device: int, path: str, cases: List[dict],
             comm.status()
             got = from_torch(y, dout)
             exact = bits_equal(got, want, dout)
-            res = dict(case=case, exact=bool(exact), ms=ms, rank=rank, kernel=comm.last_algo())
+            st = comm.stats()
+            res = dict(case=case, exact=bool(exact), ms=ms, rank=rank, kernel=comm.last_algo(),
+                       ctas=st.last_ctas)
+            if case.get("keep"):
+                res.update(got=got, want=want)
+            note = None
             if case.get("expect_kernel") and res["kernel"] != case["expect_kernel"] and \
                     not (case["expect_kernel"] == "nvls_inplace" and not caps.multicast):
+                note = "took %s, expected %s" % (res["kernel"], case["expect_kernel"])
+            elif case.get("expect_ctas") is not None and st.last_ctas != case["expect_ctas"]:
+                note = "launched %d CTAs, expected %d" % (st.last_ctas, case["expect_ctas"])
+            elif guard and not (_guards_intact(xf, guard, count) and _guards_intact(yf, guard, count)):
+                note = "wrote outside the bucket"
+            elif guard and not (symm or inplace) and \
+                    from_torch(x, din).tobytes() != np.ascontiguousarray(inputs[rank]).tobytes():
+                note = "changed the input of an out-of-place call"
+            if note:
                 res["exact"] = False
-                res["note"] = "took %s, expected %s" % (res["kernel"], case["expect_kernel"])
+                res["note"] = note
                 res.update(max_ulp=-1, mismatch=-1, normwise=-1.0)
                 results.append(res)
                 continue
@@ -184,8 +306,147 @@ def run_cases(rank: int, world: int, device: int, path: str, cases: List[dict],
                 bad = np.nonzero(ulp)[0][:4]
                 res["first_bad"] = [int(i) for i in bad]
             results.append(res)
-        res_launch = comm.launches()
-        results.append(dict(launches=res_launch, multicast=int(caps.multicast), rank=rank))
+        res_launch = comm.launches()   # arrival kernels included
+        results.append(dict(launches=res_launch, exchange_launches=comm.stats().launches,
+                            multicast=int(caps.multicast), rank=rank))
+    finally:
+        comm.close()
+    return results
+
+
+GUARD_BYTE = 0xA5
+
+
+def _guarded(alloc, count, guard, dtype):
+    """count + 2*guard elements from `alloc`, every byte GUARD_BYTE.  guard * element size must be a
+    multiple of 16 so that the middle view keeps the 16-byte alignment buckets need."""
+    import torch
+    t = alloc(count + 2 * guard, dtype)
+    assert (guard * t.element_size()) % 16 == 0
+    t.view(torch.uint8).fill_(GUARD_BYTE)
+    return t
+
+
+def _guards_intact(full, guard, count) -> bool:
+    import torch
+    b = full.view(torch.uint8).cpu().numpy()
+    es = full.element_size()
+    return bool((b[:guard * es] == GUARD_BYTE).all() and (b[(guard + count) * es:] == GUARD_BYTE).all())
+
+
+def plan_launches(count: int, din: str, dw: str, dout: str, world: int, algo: int, *,
+                  inplace: bool = False, staging_mb: int = 32, max_ctas: int = 16,
+                  cta_bytes: int = 65536) -> List[dict]:
+    """Restatement of how tok_allreduce_bucket splits a staged (algo 2 one-shot, 3 two-shot) or
+    zero-copy (inplace) bucket into launches and sizes each grid (csrc/comm.cpp): per launch the
+    element count n, total_packs, the slab length L (packs per CTA), the sub-slab M = L / world and
+    the grid size.  max_ctas stands for TOK_MAX_CTAS, which also caps the zero-copy grid when set."""
+    P = 4 if "f32" in (din, dw, dout) else 8
+    wsz = 4 if dw == "f32" else 2
+    cap_bytes = -(-(staging_mb << 20) // (2 << 20)) * (2 << 20)
+    if inplace:
+        launch_cap = count
+    else:
+        launch_cap = (cap_bytes // 8 if algo == 2 else cap_bytes) // wsz
+        launch_cap = launch_cap // (P * 8) * (P * 8)
+    out = []
+    for off in range(0, count, launch_cap):
+        n = min(launch_cap, count - off)
+        packs = -(-n // P)
+        g = min(max(-(-(packs * P * wsz) // cta_bytes), 1), max_ctas)
+        L = -(-packs // g)
+        if algo != 2:
+            L = -(-L // world) * world
+        out.append(dict(n=n, packs=packs, L=L, M=L // world, ctas=-(-packs // L), P=P))
+    return out
+
+
+def run_queued(rank: int, world: int, device: int, path: str, cases: List[dict],
+               job: str = "queued", repeats: int = 2) -> List[dict]:
+    """Body of one replica that enqueues every case on ONE stream back to back and synchronises once
+    at the end, `repeats` times over the same buffers (inputs are copied in again, on the stream,
+    before each pass).  Cases: allreduce cases as in run_cases (count / in / wire / out / scale /
+    post / algo / pattern / seed / symm / split / expect_kernel) and broadcasts (bcast=root, count
+    in bytes, symm).  Returns one result per case and pass, plus the exchange launches of each pass."""
+    import torch
+    from oracle.allreduce_oracle import allreduce_oracle, to_f32, ulp_distance
+    from torch_on_k8s_b200.comm import Communicator
+
+    torch.cuda.set_device(device)
+    dev = torch.device("cuda", device)
+    comm = Communicator(job, rank, world, device, rendezvous_path=path)
+    stream = torch.cuda.Stream(device=dev)
+    results = []
+    try:
+        prepared = []
+        with torch.cuda.stream(stream):   # every buffer first, in the same order on every replica
+            for ci, case in enumerate(cases):
+                if case.get("bcast") is not None:
+                    src = [np.random.RandomState(9000 + 13 * ci + r).randint(0, 256, case["count"],
+                                                                             dtype=np.uint8)
+                           for r in range(world)]
+                    t = comm.symm_empty(case["count"], torch.uint8) if case.get("symm") else \
+                        torch.empty(case["count"], dtype=torch.uint8, device=dev)
+                    prepared.append(dict(src=torch.from_numpy(src[rank]).to(dev), x=t, y=t,
+                                         want=src[case["bcast"]]))
+                    continue
+                din, dw, dout, count = case["in"], case["wire"], case["out"], case["count"]
+                scale, post = case.get("scale", 1.0 / world), case.get("post", False)
+                inputs = [gen_input(case.get("seed", 5000 + ci), r, count, din,
+                                    case.get("pattern", "randn")) for r in range(world)]
+                want = allreduce_oracle(inputs, din, dw, dout, scale, post)
+                if case.get("symm"):
+                    x = comm.symm_empty(count, torch_dtype(din))
+                    assert comm.in_symmetric_pool(x)
+                else:
+                    x = torch.empty(count, dtype=torch_dtype(din), device=dev)
+                y = x if case.get("inplace", din == dout) else \
+                    torch.empty(count, dtype=torch_dtype(dout), device=dev)
+                prepared.append(dict(src=to_torch(inputs[rank], din, dev), x=x, y=y, want=want))
+        stream.synchronize()
+        for rep in range(repeats):
+            launches0 = comm.stats().launches
+            kernels = []
+            with torch.cuda.stream(stream):
+                for case, p in zip(cases, prepared):
+                    p["x"].copy_(p["src"])
+                    if case.get("bcast") is not None:
+                        comm.broadcast(p["x"], case["bcast"], stream=stream)
+                    else:
+                        scale, post = case.get("scale", 1.0 / world), case.get("post", False)
+                        algo = case.get("algo", 0)
+                        arrived = False
+                        if case.get("split"):
+                            arrived = comm.bucket_arrive(p["x"], scale=scale, post_scale=post,
+                                                         algo=algo, stream=stream)
+                        comm.allreduce_bucket(p["x"], p["y"], scale=scale,
+                                              wire_dtype=torch_dtype(case["wire"]), post_scale=post,
+                                              algo=algo, arrived=arrived, stream=stream)
+                    kernels.append(comm.last_algo())
+            stream.synchronize()
+            comm.status()
+            launches = comm.stats().launches - launches0
+            for case, p, kernel in zip(cases, prepared, kernels):
+                res = dict(case=case, rank=rank, kernel=kernel, rep=rep)
+                if case.get("bcast") is not None:
+                    got = p["y"].cpu().numpy()
+                    res["mismatch"] = int((got != p["want"]).sum())
+                    res["exact"] = res["mismatch"] == 0
+                else:
+                    got = from_torch(p["y"], case["out"])
+                    res["exact"] = bits_equal(got, p["want"], case["out"])
+                    if not res["exact"]:
+                        ulp = ulp_distance(got, p["want"], case["out"])
+                        both_nan = np.isnan(to_f32(got, case["out"])) & \
+                            np.isnan(to_f32(p["want"], case["out"]))
+                        ulp = np.where(both_nan, 0, ulp)
+                        res.update(max_ulp=int(ulp.max()), mismatch=int((ulp != 0).sum()),
+                                   first_bad=[int(i) for i in np.nonzero(ulp)[0][:4]])
+                if case.get("expect_kernel") and kernel != case["expect_kernel"]:
+                    res["exact"] = False
+                    res["note"] = "took %s, expected %s" % (kernel, case["expect_kernel"])
+                results.append(res)
+            results.append(dict(launches=launches, rep=rep, rank=rank))
     finally:
         comm.close()
     return results
@@ -246,18 +507,19 @@ def _run_golden(comm, case, rank, world, dev, stream):
                 max_ulp=int(ulp.max()), mismatch=int((ulp != 0).sum()))
 
 
-def _proc_entry(rank, world, device, path, cases, job, env, q):
+def _proc_entry(rank, world, device, path, cases, job, env, q, body=None):
     try:
         os.environ.update(env or {})
-        q.put((rank, "ok", run_cases(rank, world, device, path, cases, job)))
+        q.put((rank, "ok", (body or run_cases)(rank, world, device, path, cases, job)))
     except Exception:  # noqa: BLE001
         q.put((rank, "error", traceback.format_exc()))
 
 
 def launch(world: int, cases: List[dict], *, devices: Optional[List[int]] = None,
            mode: str = "proc", timeout: float = 300.0, env: Optional[Dict[str, str]] = None,
-           job: str = "harness") -> Dict[int, list]:
-    """Run `cases` on `world` replicas; returns {rank: results}.  Raises on replica failure."""
+           job: str = "harness", body=None) -> Dict[int, list]:
+    """Run `cases` on `world` replicas; returns {rank: results}.  Raises on replica failure.
+    body: the replica body for mode "proc" (default run_cases; run_queued for queued sequences)."""
     devices = devices or [0] * world
     tmp = tempfile.mkdtemp(prefix="tok8s-")
     path = os.path.join(tmp, "rdzv")
@@ -266,7 +528,7 @@ def launch(world: int, cases: List[dict], *, devices: Optional[List[int]] = None
         ctx = mp.get_context("spawn")
         q = ctx.Queue()
         procs = [ctx.Process(target=_proc_entry,
-                             args=(r, world, devices[r], path, cases, job, env, q), daemon=True)
+                             args=(r, world, devices[r], path, cases, job, env, q, body), daemon=True)
                  for r in range(world)]
         for p in procs:
             p.start()
@@ -297,6 +559,7 @@ def launch(world: int, cases: List[dict], *, devices: Optional[List[int]] = None
         if errors:
             raise RuntimeError("replica %d failed:\n%s" % errors[0])
     elif mode == "thread":
+        assert body is None, "thread-mode replicas run run_cases"
         if env:
             os.environ.update(env)
         errs = []

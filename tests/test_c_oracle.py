@@ -58,6 +58,83 @@ def test_c_oracle_equals_numpy_oracle(clib, world, post):
                     assert harness.bits_equal(got, want, dout), (din, dw, dout, pattern)
 
 
+def torch_allreduce(inputs, din, dw, dout, scale, post):
+    """A third restatement of the oracle, in torch CPU float32 ops and torch's own dtype casts."""
+    import torch
+    tdt = {"f32": torch.float32, "bf16": torch.bfloat16, "f16": torch.float16}
+
+    def load(a, dt):
+        if dt == "bf16":
+            return torch.from_numpy(a.view(np.int16).copy()).view(torch.bfloat16).float()
+        return torch.from_numpy(a.copy()).float()
+
+    pre = torch.tensor(1.0 if post else scale, dtype=torch.float32)
+    pst = torch.tensor(scale if post else 1.0, dtype=torch.float32)
+    acc = None
+    for a in inputs:
+        w = (load(a, din) * pre).to(tdt[dw]).float()
+        acc = w if acc is None else acc + w
+    out = (acc * pst).to(tdt[dw]).float().to(tdt[dout])
+    if dout == "bf16":
+        return out.view(torch.int16).numpy().view(np.uint16)
+    return out.numpy()
+
+
+@pytest.mark.filterwarnings("ignore:overflow encountered:RuntimeWarning")
+@pytest.mark.parametrize("world", range(1, 9))
+def test_special_values_three_oracles_agree(clib, world):
+    """On the edge-value pattern (signed zeros, inf, NaN, overflow, subnormals, rounding ties,
+    order-sensitive sums) the numpy oracle, the C oracle and a torch restatement give the same bits
+    for every dtype triple and scale, NaN payloads aside."""
+    seed = 300 + 50 * world
+    for din in O.DTYPES:
+        for dw in O.DTYPES:
+            for dout in O.DTYPES:
+                for scale, post in harness.special_scales(world):
+                    seed += 1
+                    n = 31 * 8 + 3 + seed % 5
+                    ins = [harness.gen_input(seed, r, n, din, "special") for r in range(world)]
+                    s32 = float(np.float32(scale))
+                    want = O.allreduce_oracle(ins, din, dw, dout, s32, post)
+                    got_c = c_allreduce(clib, ins, din, dw, dout, s32, post)
+                    got_t = torch_allreduce(ins, din, dw, dout, s32, post)
+                    what = (din, dw, dout, scale, post)
+                    assert harness.bits_equal(got_c, want, dout), what
+                    assert harness.bits_equal(got_t, want, dout), what
+
+
+def test_special_pattern_produces_every_recipe():
+    """The edge-value generator puts every recipe in every lane of a 4- and an 8-element pack and
+    produces, for every in dtype: -0, +inf, -inf, NaN, the dtype's largest finite value, its smallest
+    subnormal and both fp32 overflow thresholds of the wire casts (f32 inputs)."""
+    from oracle.allreduce_oracle import to_f32
+    n = 4099
+    idx, _ = harness.special_layout(77, n)
+    for k in range(len(harness.SPECIAL_RECIPES)):
+        lanes = set(np.nonzero(idx == k)[0] % 8)
+        assert lanes == set(range(8)), (harness.SPECIAL_RECIPES[k][0], lanes)
+    assert (idx == -1).any()                                        # the randn background stays
+    smallest = {"f32": 2.0 ** -149, "bf16": 2.0 ** -133, "f16": 2.0 ** -24}
+    for dt in O.DTYPES:
+        v = np.concatenate([to_f32(harness.gen_input(77, r, n, dt, "special"), dt) for r in range(3)])
+        bits = v.view(np.uint32)
+        assert (bits == 0x80000000).any() and (bits == 0).any()
+        assert np.isposinf(v).any() and np.isneginf(v).any() and np.isnan(v).any()
+        assert (v == to_f32(O.from_f32(harness._MAX[dt].reshape(1), dt), dt)[0]).any()
+        assert (v == np.float32(smallest[dt])).any(), dt
+        sub = (v != 0) & (np.abs(v) < {"f32": 2.0 ** -126, "bf16": 2.0 ** -126, "f16": 2.0 ** -14}[dt])
+        assert sub.any(), dt
+    v = harness.gen_input(77, 0, n, "f32", "special")
+    for bits in (0x7F7F7FFF, 0x7F7F8000, 0x7F7F8001):
+        assert (v.view(np.uint32) == bits).any()
+    assert (v == np.float32(65520.0)).any() and (v == np.nextafter(np.float32(65520), np.float32(0))).any()
+    # the order-sensitive triple: rank order gives 0, the reverse order does not
+    k = harness.SPECIAL_INDEX["order_triple"]
+    i = int(np.nonzero(idx == k)[0][0])
+    t = [harness.gen_input(77, r, n, "f32", "special")[i] for r in range(3)]
+    assert (t[0] + t[1]) + t[2] == 0 and (t[2] + t[1]) + t[0] != 0
+
+
 def test_c_conversions_match_numpy(clib):
     rs = np.random.RandomState(1)
     x = (rs.standard_normal(50000) * np.exp(rs.uniform(-30, 15, 50000))).astype(np.float32)

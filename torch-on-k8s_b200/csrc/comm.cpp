@@ -1282,7 +1282,17 @@ int plan_bucket(const tok_comm* c, const void* in, const void* out, size_t count
   const bool same_dt = in_dtype == wire_dtype && wire_dtype == out_dtype;
   int algo = static_cast<int>((flags & TOK_FLAG_ALGO_MASK) >> TOK_FLAG_ALGO_SHIFT);
   const bool forced = algo != TOK_ALGO_AUTO;
+  const bool post = (flags & TOK_FLAG_SCALE_POST) != 0;
   if (algo == TOK_ALGO_AUTO) algo = pick_algo(c, count * wsz);
+  // The switch returns the sum already rounded to the wire dtype, so a POST scale rounds a second
+  // time: exact for a power-of-two factor on a bf16 wire, 1 ulp off for other factors, and an f16
+  // sum can overflow before the factor brings it back into range.  AUTO keeps such buckets on the
+  // P2P kernels, which round once (staged: two-shot; pool buckets: two-shot in place, below).
+  // `forced` is an algorithm in the call's flags; TOK_ALGO in the environment only replaces
+  // pick_algo's choice by size and stays under this rule, as under the pool-bucket rule below.
+  if (!forced && algo == TOK_ALGO_NVLS && post && wire_dtype != TOK_F32 &&
+      (wire_dtype == TOK_F16 || !is_pow2_scale(scale)))
+    algo = TOK_ALGO_TWO_SHOT;
   if (algo == TOK_ALGO_LOCAL_TMA) {
     if (c->world != 1 || !same_dt)
       return fail(TOK_ERR_INVALID, "TOK_ALGO_LOCAL_TMA needs world == 1 and one dtype");
@@ -1316,10 +1326,10 @@ int plan_bucket(const tok_comm* c, const void* in, const void* out, size_t count
   bool inplace = pool_ok && (algo == TOK_ALGO_TWO_SHOT || algo == TOK_ALGO_NVLS);
   if (inplace) {
     // The switch can only scale the SUM.  That equals the specified PRE semantics (scale every
-    // contribution, then sum) when the caller asked for POST or the factor is a power of two; a
-    // 16-bit float sum may also overflow before the 1/N is applied.  Everything else takes the P2P
-    // in-place kernel, which applies PRE exactly as the staged path does.
-    const bool post = (flags & TOK_FLAG_SCALE_POST) != 0;
+    // contribution, then sum) when the factor is a power of two; a 16-bit float sum may also
+    // overflow before the 1/N is applied.  POST buckets that reach this point are either forced or
+    // passed the rule above.  Everything else takes the P2P in-place kernel, which applies PRE
+    // exactly as the staged path does.
     const bool nvls_exact = (post || is_pow2_scale(scale)) && (wire_dtype != TOK_F16 || post);
     // (pick_algo's rule stands for pool buckets too: with 3-4 replicas the in-switch reduction stops
     // paying off past ~12 MiB — P2P reduce+push beat NVLS in place at N=4 on the 22.9 / 28.3 MB DDP
