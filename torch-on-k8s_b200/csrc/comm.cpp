@@ -43,22 +43,24 @@ namespace tok {
 // ------------------------------------------------------------------------------------------------
 static thread_local std::string g_err;
 
-void set_error(const char* fmt, ...) {
+static void vset_error(const char* fmt, va_list ap) {
   char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
   vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
   g_err = buf;
 }
 
-int fail(int code, const char* fmt, ...) {
-  char buf[1024];
+void set_error(const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
+  vset_error(fmt, ap);
   va_end(ap);
-  g_err = buf;
+}
+
+int fail(int code, const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  vset_error(fmt, ap);
+  va_end(ap);
   return code;
 }
 
@@ -184,6 +186,21 @@ struct Hello {
   char job[64];
 };
 
+// Owns one descriptor of a heap or multicast handle (exported by the driver or received from a
+// peer) and closes it when it goes out of scope, on every exit path.
+struct Fd {
+  int fd = -1;
+  Fd() = default;
+  Fd(Fd&& o) noexcept : fd(o.fd) { o.fd = -1; }
+  Fd& operator=(Fd&& o) noexcept {
+    std::swap(fd, o.fd);
+    return *this;
+  }
+  ~Fd() {
+    if (fd >= 0) close(fd);
+  }
+};
+
 static int wait_fd(int fd, short events, double deadline) {
   for (;;) {
     double left = deadline - now_s();
@@ -230,8 +247,9 @@ static int send_msg(int sock, const void* buf, size_t len, const int* fds, int n
   return 0;
 }
 
-// Receives exactly len bytes; descriptors that arrive with them are appended to fds_out.
-static int recv_msg(int sock, void* buf, size_t len, std::vector<int>* fds_out, double deadline) {
+// Receives exactly len bytes; descriptors that arrive with them are appended to fds_out (closed
+// when fds_out is null).
+static int recv_msg(int sock, void* buf, size_t len, std::vector<Fd>* fds_out, double deadline) {
   char* p = static_cast<char*>(buf);
   size_t got = 0;
   while (got < len) {
@@ -254,12 +272,9 @@ static int recv_msg(int sock, void* buf, size_t len, std::vector<int>* fds_out, 
       if (c->cmsg_level == SOL_SOCKET && c->cmsg_type == SCM_RIGHTS) {
         int cnt = static_cast<int>((c->cmsg_len - CMSG_LEN(0)) / sizeof(int));
         for (int i = 0; i < cnt; ++i) {
-          int fd;
-          memcpy(&fd, CMSG_DATA(c) + i * sizeof(int), sizeof(int));
-          if (fds_out)
-            fds_out->push_back(fd);
-          else
-            close(fd);
+          Fd fd;
+          memcpy(&fd.fd, CMSG_DATA(c) + i * sizeof(int), sizeof(int));
+          if (fds_out) fds_out->push_back(std::move(fd));
         }
       }
     }
@@ -326,7 +341,6 @@ struct PeerMap {
   uint64_t uid = 0;
   CUmemGenericAllocationHandle handle = 0;
   CUdeviceptr va = 0;
-  bool own = false;
 };
 
 struct tok_comm {
@@ -351,7 +365,7 @@ struct tok_comm {
   CUmemGenericAllocationHandle local_handle = 0;
   CUdeviceptr local_va = 0;
 
-  std::vector<PeerMap> cache;      // every heap currently mapped (including our own)
+  std::vector<PeerMap> cache;      // every peer heap currently imported and mapped (not our own)
   char* peer[kMaxWorld] = {0};     // by current rank
 
   bool mc_bound = false;
@@ -404,12 +418,23 @@ struct DeviceGuard {
   }
 };
 
+// Gives back a heap-sized VA range reserved by map_heap() and clears *va.  `mapped` is false only
+// for a reservation whose cuMemMap failed.
+void unmap(tok_comm* c, CUdeviceptr* va, bool mapped = true) {
+  if (!*va) return;
+  if (mapped) drv().cuMemUnmap_(*va, c->heap_bytes);
+  drv().cuMemAddressFree_(*va, c->heap_bytes);
+  *va = 0;
+}
+
+// Maps a heap-sized handle (our own heap, a peer's heap, or the multicast object) read-write for
+// this replica's GPU.  On failure *va is 0 and nothing is left reserved.
 int map_heap(tok_comm* c, CUmemGenericAllocationHandle h, CUdeviceptr* va) {
   Drv& d = drv();
   CU_CHECK(d.cuMemAddressReserve_(va, c->heap_bytes, c->gran, 0, 0));
   CUresult r = d.cuMemMap_(*va, c->heap_bytes, 0, h, 0);
   if (r != CUDA_SUCCESS) {
-    d.cuMemAddressFree_(*va, c->heap_bytes);
+    unmap(c, va, false);
     return fail(TOK_ERR_CUDA, "cuMemMap failed: %s", cu_err(r));
   }
   CUmemAccessDesc acc;
@@ -419,8 +444,7 @@ int map_heap(tok_comm* c, CUmemGenericAllocationHandle h, CUdeviceptr* va) {
   acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
   r = d.cuMemSetAccess_(*va, c->heap_bytes, &acc, 1);
   if (r != CUDA_SUCCESS) {
-    d.cuMemUnmap_(*va, c->heap_bytes);
-    d.cuMemAddressFree_(*va, c->heap_bytes);
+    unmap(c, va);
     return fail(TOK_ERR_CUDA,
                 "cuMemSetAccess on a peer heap failed: %s (no P2P path between the replicas' GPUs?)",
                 cu_err(r));
@@ -428,23 +452,15 @@ int map_heap(tok_comm* c, CUmemGenericAllocationHandle h, CUdeviceptr* va) {
   return TOK_OK;
 }
 
-void unmap_heap(tok_comm* c, PeerMap& m) {
-  Drv& d = drv();
-  if (m.va) {
-    d.cuMemUnmap_(m.va, c->heap_bytes);
-    d.cuMemAddressFree_(m.va, c->heap_bytes);
-  }
-  if (m.handle && !m.own) d.cuMemRelease_(m.handle);
+void release_peer(tok_comm* c, PeerMap& m) {
+  unmap(c, &m.va);
+  if (m.handle) drv().cuMemRelease_(m.handle);
   m = PeerMap();
 }
 
 void teardown_multicast(tok_comm* c) {
   Drv& d = drv();
-  if (c->mc_va) {
-    d.cuMemUnmap_(c->mc_va, c->heap_bytes);
-    d.cuMemAddressFree_(c->mc_va, c->heap_bytes);
-    c->mc_va = 0;
-  }
+  unmap(c, &c->mc_va);
   if (c->mc_handle) {
     if (c->mc_bound) d.cuMulticastUnbind_(c->mc_handle, c->cu_dev, 0, c->heap_bytes);
     d.cuMemRelease_(c->mc_handle);
@@ -504,21 +520,12 @@ int alloc_local(tok_comm* c) {
   void* dp = nullptr;
   RT_CHECK(cudaHostGetDevicePointer(&dp, hp, 0));
   c->hostctl_dev = static_cast<uint32_t*>(dp);
-  PeerMap self;
-  self.uid = c->uid;
-  self.handle = c->local_handle;
-  self.va = c->local_va;
-  self.own = true;
-  c->cache.push_back(self);
   return TOK_OK;
 }
 
-// One membership exchange: gathers every member's Hello + heap fd at the group's rank 0 and
-// scatters the full table back, then (re)builds the peer table and the multicast binding.
-int exchange(tok_comm* c) {
-  Drv& d = drv();
-  c->membership_dirty = false;
-  Star star;
+// Step 1 of an exchange: gathers every member's Hello + heap fd at the group's rank 0 and scatters
+// the full table, with every member's fd, back.  `star` keeps the group's sockets for later steps.
+int rendezvous(tok_comm* c, Star& star, std::vector<Hello>& table, std::vector<Fd>& fds) {
   star.root = (c->rank == 0);
   star.world = c->world;
   star.deadline = now_s() + c->rdzv_timeout_s;
@@ -562,57 +569,39 @@ int exchange(tok_comm* c) {
   memcpy(me.bus_id, c->bus_id, sizeof(me.bus_id));
   snprintf(me.job, sizeof(me.job), "%s", c->job_id.c_str());
 
-  std::vector<Hello> table(c->world);
-  std::vector<int> fds(c->world, -1);
-  auto close_fds = [&] {
-    for (int& f : fds)
-      if (f >= 0) {
-        close(f);
-        f = -1;
-      }
-  };
-
-  int my_fd = -1;
+  Fd my_fd;
   if (c->world > 1)
-    CU_CHECK(d.cuMemExportToShareableHandle_(&my_fd, c->local_handle,
-                                             CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0));
+    CU_CHECK(drv().cuMemExportToShareableHandle_(&my_fd.fd, c->local_handle,
+                                                 CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0));
 
   if (c->world == 1) {
     table[0] = me;
   } else if (star.root) {
     star.listen_fd = socket(AF_UNIX, SOCK_STREAM | SOCK_CLOEXEC, 0);
-    if (star.listen_fd < 0) {
-      close(my_fd);
-      return fail(TOK_ERR_RENDEZVOUS, "socket(): %s", strerror(errno));
-    }
+    if (star.listen_fd < 0) return fail(TOK_ERR_RENDEZVOUS, "socket(): %s", strerror(errno));
     if (!abstract_sock) unlink(star.path.c_str());
     if (bind(star.listen_fd, reinterpret_cast<struct sockaddr*>(&addr), sizeof(addr)) != 0 ||
-        listen(star.listen_fd, kMaxWorld) != 0) {
-      close(my_fd);
+        listen(star.listen_fd, kMaxWorld) != 0)
       return fail(TOK_ERR_RENDEZVOUS, "bind/listen(%s): %s", star.path.c_str(), strerror(errno));
-    }
     star.conn.assign(c->world, -1);
     table[0] = me;
-    fds[0] = my_fd;
+    fds.resize(c->world);
+    fds[0] = std::move(my_fd);
     for (int joined = 1; joined < c->world; ++joined) {
-      if (wait_fd(star.listen_fd, POLLIN, star.deadline) <= 0) {
-        close_fds();
+      if (wait_fd(star.listen_fd, POLLIN, star.deadline) <= 0)
         return fail(TOK_ERR_RENDEZVOUS,
                     "rendezvous %s: only %d of %d replicas joined within %.0f s", star.path.c_str(),
                     joined, c->world, c->rdzv_timeout_s);
-      }
       int s = accept4(star.listen_fd, nullptr, nullptr, SOCK_CLOEXEC);
       if (s < 0) {
         --joined;
         continue;
       }
       Hello h;
-      std::vector<int> got;
+      std::vector<Fd> got;
       if (recv_msg(s, &h, sizeof(h), &got, star.deadline) != 0 || h.magic != kMagic ||
           got.size() != 1) {
-        for (int f : got) close(f);
         close(s);
-        close_fds();
         return fail(TOK_ERR_RENDEZVOUS, "rendezvous %s: malformed hello", star.path.c_str());
       }
       const bool bad = h.abi != TOK_ABI_VERSION || h.epoch != c->epoch || h.world != c->world ||
@@ -620,9 +609,7 @@ int exchange(tok_comm* c) {
                        h.heap_bytes != c->heap_bytes || h.cap_bytes != c->cap_bytes ||
                        strncmp(h.job, me.job, sizeof(h.job)) != 0;
       if (bad) {
-        close(got[0]);
         close(s);
-        close_fds();
         return fail(TOK_ERR_RENDEZVOUS,
                     "rendezvous %s: replica rank=%d world=%d epoch=%llu heap=%llu job=%.63s does not "
                     "match this group (world=%d epoch=%llu heap=%llu job=%s)",
@@ -632,85 +619,73 @@ int exchange(tok_comm* c) {
       }
       star.conn[h.rank] = s;
       table[h.rank] = h;
-      fds[h.rank] = got[0];
+      fds[h.rank] = std::move(got[0]);
     }
-    for (int r = 1; r < c->world; ++r) {
-      if (send_msg(star.conn[r], table.data(), sizeof(Hello) * c->world, fds.data(), c->world,
-                   star.deadline) != 0) {
-        close_fds();
+    std::vector<int> raw;
+    for (const Fd& f : fds) raw.push_back(f.fd);
+    for (int r = 1; r < c->world; ++r)
+      if (send_msg(star.conn[r], table.data(), sizeof(Hello) * c->world, raw.data(), c->world,
+                   star.deadline) != 0)
         return fail(TOK_ERR_RENDEZVOUS, "rendezvous: cannot send the table to rank %d", r);
-      }
-    }
   } else {
     int s = -1;
     for (;;) {
       s = socket(AF_UNIX, SOCK_STREAM | SOCK_CLOEXEC, 0);
-      if (s < 0) {
-        close(my_fd);
-        return fail(TOK_ERR_RENDEZVOUS, "socket(): %s", strerror(errno));
-      }
+      if (s < 0) return fail(TOK_ERR_RENDEZVOUS, "socket(): %s", strerror(errno));
       if (connect(s, reinterpret_cast<struct sockaddr*>(&addr), sizeof(addr)) == 0) break;
       close(s);
-      if (now_s() > star.deadline) {
-        close(my_fd);
+      if (now_s() > star.deadline)
         return fail(TOK_ERR_RENDEZVOUS, "rendezvous %s: the group root never appeared (%.0f s)",
                     star.path.c_str(), c->rdzv_timeout_s);
-      }
       usleep(20000);
     }
     star.conn.assign(1, s);
-    int rc = send_msg(s, &me, sizeof(me), &my_fd, 1, star.deadline);
-    close(my_fd);
-    my_fd = -1;
-    if (rc != 0) return fail(TOK_ERR_RENDEZVOUS, "rendezvous: cannot send hello");
-    std::vector<int> got;
-    if (recv_msg(s, table.data(), sizeof(Hello) * c->world, &got, star.deadline) != 0 ||
-        static_cast<int>(got.size()) != c->world) {
-      for (int f : got) close(f);
+    if (send_msg(s, &me, sizeof(me), &my_fd.fd, 1, star.deadline) != 0)
+      return fail(TOK_ERR_RENDEZVOUS, "rendezvous: cannot send hello");
+    if (recv_msg(s, table.data(), sizeof(Hello) * c->world, &fds, star.deadline) != 0 ||
+        static_cast<int>(fds.size()) != c->world)
       return fail(TOK_ERR_RENDEZVOUS,
                   "rendezvous %s: no membership table from the root (it rejected this replica or "
                   "timed out)",
                   star.path.c_str());
-    }
-    for (int r = 0; r < c->world; ++r) fds[r] = got[r];
   }
+  return TOK_OK;
+}
 
-  // ---- build the peer table, reusing mappings of surviving peers (in-place re-form) -------------
+// Step 2: the peer table of the new membership.  Mappings of surviving peers are reused (in-place
+// re-form), new peers' heaps are imported from their fds, dropped peers' heaps are released.
+int rebuild_peers(tok_comm* c, Star& star, const std::vector<Hello>& table, std::vector<Fd> fds) {
+  Drv& d = drv();
   c->membership_dirty = true;
   std::vector<PeerMap> next;
   int rc = TOK_OK;
   for (int r = 0; r < c->world && rc == TOK_OK; ++r) {
+    if (table[r].uid == c->uid) continue;
     auto it = std::find_if(c->cache.begin(), c->cache.end(),
                            [&](const PeerMap& m) { return m.uid == table[r].uid && m.va != 0; });
     if (it != c->cache.end()) {
       next.push_back(*it);
-      it->va = 0;  // moved
-      it->handle = 0;
-    } else {
-      PeerMap m;
-      m.uid = table[r].uid;
-      CUresult cr = d.cuMemImportFromShareableHandle_(
-          &m.handle, reinterpret_cast<void*>(static_cast<uintptr_t>(fds[r])),
-          CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
-      if (cr != CUDA_SUCCESS) {
-        rc = fail(TOK_ERR_CUDA, "cuMemImportFromShareableHandle(rank %d) failed: %s", r, cu_err(cr));
-        break;
-      }
-      rc = map_heap(c, m.handle, &m.va);
-      if (rc != TOK_OK) {
-        d.cuMemRelease_(m.handle);
-        break;
-      }
-      next.push_back(m);
+      *it = PeerMap();  // moved
+      continue;
     }
+    PeerMap m;
+    m.uid = table[r].uid;
+    CUresult cr = d.cuMemImportFromShareableHandle_(
+        &m.handle, reinterpret_cast<void*>(static_cast<uintptr_t>(fds[r].fd)),
+        CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
+    if (cr != CUDA_SUCCESS) {
+      rc = fail(TOK_ERR_CUDA, "cuMemImportFromShareableHandle(rank %d) failed: %s", r, cu_err(cr));
+      break;
+    }
+    rc = map_heap(c, m.handle, &m.va);
+    if (rc != TOK_OK) {
+      d.cuMemRelease_(m.handle);
+      break;
+    }
+    next.push_back(m);
   }
-  close_fds();
-  // whatever is left in the old cache belongs to replicas that were dropped (never our own heap:
-  // our uid is always in the table)
-  for (PeerMap& m : c->cache)
-    if (m.va != 0 && !m.own) unmap_heap(c, m);
-  for (PeerMap& m : c->cache)
-    if (m.va != 0 && m.own) next.push_back(m);  // only reachable after a failed exchange
+  // whatever is left in the old cache belongs to replicas that were dropped
+  for (PeerMap& m : c->cache) release_peer(c, m);
   c->cache.swap(next);
   int all = 0;
   int brc = c->world > 1 ? star.all_ok(rc == TOK_OK, &all) : (all = (rc == TOK_OK), TOK_OK);
@@ -718,13 +693,17 @@ int exchange(tok_comm* c) {
   if (brc != TOK_OK) return brc;
   if (!all) return fail(TOK_ERR_RENDEZVOUS, "a peer failed to map the group's heaps");
   for (int r = 0; r < kMaxWorld; ++r) c->peer[r] = reinterpret_cast<char*>(c->local_va);
-  for (int r = 0; r < c->world; ++r) {
-    auto it = std::find_if(c->cache.begin(), c->cache.end(),
-                           [&](const PeerMap& m) { return m.uid == table[r].uid; });
-    c->peer[r] = reinterpret_cast<char*>(it->va);
-  }
+  for (const PeerMap& m : c->cache)
+    for (int r = 0; r < c->world; ++r)
+      if (table[r].uid == m.uid) c->peer[r] = reinterpret_cast<char*>(m.va);
+  return TOK_OK;
+}
 
-  // ---- NVSwitch multicast (NVLS) -----------------------------------------------------------------
+// Step 3: binds every member's heap to one NVSwitch multicast object (NVLS) in three agreement
+// rounds: every GPU added, every heap bound, every member mapped.  NVLS is optional: unless a
+// socket is lost, a failure leaves the group on the P2P algorithms.
+int bind_multicast(tok_comm* c, Star& star, const std::vector<Hello>& table) {
+  Drv& d = drv();
   teardown_multicast(c);
   bool mc_possible = c->world > 1;
   for (int r = 0; r < c->world; ++r) {
@@ -733,96 +712,73 @@ int exchange(tok_comm* c) {
       if (strncmp(table[r].bus_id, table[q].bus_id, sizeof(table[r].bus_id)) == 0)
         mc_possible = false;  // two replicas share a GPU (single-GPU test mode)
   }
-  if (mc_possible) {
-    int ok = 1;
-    int mc_fd = -1;
-    if (star.root) {
-      CUmulticastObjectProp mp;
-      memset(&mp, 0, sizeof(mp));
-      mp.numDevices = static_cast<unsigned>(c->world);
-      mp.size = c->heap_bytes;
-      mp.handleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
-      CUresult cr = d.cuMulticastCreate_(&c->mc_handle, &mp);
-      if (cr == CUDA_SUCCESS)
-        cr = d.cuMemExportToShareableHandle_(&mc_fd, c->mc_handle,
-                                             CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0);
+  if (!mc_possible) return TOK_OK;
+  int ok = 1;
+  if (star.root) {
+    Fd mc_fd;
+    CUmulticastObjectProp mp;
+    memset(&mp, 0, sizeof(mp));
+    mp.numDevices = static_cast<unsigned>(c->world);
+    mp.size = c->heap_bytes;
+    mp.handleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
+    CUresult cr = d.cuMulticastCreate_(&c->mc_handle, &mp);
+    if (cr == CUDA_SUCCESS)
+      cr = d.cuMemExportToShareableHandle_(&mc_fd.fd, c->mc_handle,
+                                           CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0);
+    if (cr != CUDA_SUCCESS) {
+      set_error("multicast create/export failed: %s", cu_err(cr));
+      ok = 0;
+    }
+    for (int r = 1; r < c->world; ++r) {
+      int32_t hdr = ok;
+      if (send_msg(star.conn[r], &hdr, sizeof(hdr), ok ? &mc_fd.fd : nullptr, ok ? 1 : 0,
+                   star.deadline) != 0)
+        return fail(TOK_ERR_RENDEZVOUS, "rendezvous: cannot send the multicast handle");
+    }
+  } else {
+    int32_t hdr = 0;
+    std::vector<Fd> got;
+    if (recv_msg(star.conn[0], &hdr, sizeof(hdr), &got, star.deadline) != 0)
+      return fail(TOK_ERR_RENDEZVOUS, "rendezvous: no multicast handle from the root");
+    ok = hdr && got.size() == 1;
+    if (ok) {
+      CUresult cr = d.cuMemImportFromShareableHandle_(
+          &c->mc_handle, reinterpret_cast<void*>(static_cast<uintptr_t>(got[0].fd)),
+          CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
       if (cr != CUDA_SUCCESS) {
-        set_error("multicast create/export failed: %s", cu_err(cr));
+        set_error("multicast import failed: %s", cu_err(cr));
+        c->mc_handle = 0;
         ok = 0;
       }
-      for (int r = 1; r < c->world; ++r) {
-        int32_t hdr = ok;
-        if (send_msg(star.conn[r], &hdr, sizeof(hdr), ok ? &mc_fd : nullptr, ok ? 1 : 0,
-                     star.deadline) != 0)
-          return fail(TOK_ERR_RENDEZVOUS, "rendezvous: cannot send the multicast handle");
-      }
-      if (mc_fd >= 0) close(mc_fd);
-    } else {
-      int32_t hdr = 0;
-      std::vector<int> got;
-      if (recv_msg(star.conn[0], &hdr, sizeof(hdr), &got, star.deadline) != 0)
-        return fail(TOK_ERR_RENDEZVOUS, "rendezvous: no multicast handle from the root");
-      ok = hdr;
-      if (ok && got.size() == 1) {
-        CUresult cr = d.cuMemImportFromShareableHandle_(
-            &c->mc_handle, reinterpret_cast<void*>(static_cast<uintptr_t>(got[0])),
-            CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
-        if (cr != CUDA_SUCCESS) {
-          set_error("multicast import failed: %s", cu_err(cr));
-          c->mc_handle = 0;
-          ok = 0;
-        }
-      } else {
-        ok = 0;
-      }
-      for (int f : got) close(f);
     }
-    if (ok && d.cuMulticastAddDevice_(c->mc_handle, c->cu_dev) != CUDA_SUCCESS) ok = 0;
-    int all_added = 0;
-    rc = star.all_ok(ok, &all_added);
-    if (rc != TOK_OK) return rc;
-    int bound = 0;
-    if (all_added) {
-      CUresult cr = d.cuMulticastBindMem_(c->mc_handle, 0, c->local_handle, 0, c->heap_bytes, 0);
-      if (cr == CUDA_SUCCESS) {
-        c->mc_bound = true;
-        bound = 1;
-      } else {
-        set_error("cuMulticastBindMem failed: %s", cu_err(cr));
-      }
-    }
-    int all_bound = 0;
-    rc = star.all_ok(bound, &all_bound);
-    if (rc != TOK_OK) return rc;
-    int mapped = 0;
-    if (all_bound) {
-      CUdeviceptr va = 0;
-      if (d.cuMemAddressReserve_(&va, c->heap_bytes, c->gran, 0, 0) == CUDA_SUCCESS) {
-        CUmemAccessDesc acc;
-        memset(&acc, 0, sizeof(acc));
-        acc.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-        acc.location.id = c->cu_dev;
-        acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-        if (d.cuMemMap_(va, c->heap_bytes, 0, c->mc_handle, 0) == CUDA_SUCCESS) {
-          if (d.cuMemSetAccess_(va, c->heap_bytes, &acc, 1) == CUDA_SUCCESS) {
-            c->mc_va = va;
-            mapped = 1;
-          } else {
-            d.cuMemUnmap_(va, c->heap_bytes);
-            d.cuMemAddressFree_(va, c->heap_bytes);
-          }
-        } else {
-          d.cuMemAddressFree_(va, c->heap_bytes);
-        }
-      }
-    }
-    int all_mapped = 0;
-    rc = star.all_ok(mapped, &all_mapped);
-    if (rc != TOK_OK) return rc;
-    if (!all_mapped) teardown_multicast(c);  // NVLS is optional: fall back to P2P algorithms
   }
+  if (ok && d.cuMulticastAddDevice_(c->mc_handle, c->cu_dev) != CUDA_SUCCESS) ok = 0;
+  int all_added = 0;
+  int rc = star.all_ok(ok, &all_added);
+  if (rc != TOK_OK) return rc;
+  int bound = 0;
+  if (all_added) {
+    CUresult cr = d.cuMulticastBindMem_(c->mc_handle, 0, c->local_handle, 0, c->heap_bytes, 0);
+    if (cr == CUDA_SUCCESS) {
+      c->mc_bound = true;
+      bound = 1;
+    } else {
+      set_error("cuMulticastBindMem failed: %s", cu_err(cr));
+    }
+  }
+  int all_bound = 0;
+  rc = star.all_ok(bound, &all_bound);
+  if (rc != TOK_OK) return rc;
+  const int mapped = all_bound && map_heap(c, c->mc_handle, &c->mc_va) == TOK_OK;
+  int all_mapped = 0;
+  rc = star.all_ok(mapped, &all_mapped);
+  if (rc != TOK_OK) return rc;
+  if (!all_mapped) teardown_multicast(c);  // NVLS is optional: fall back to P2P algorithms
+  return TOK_OK;
+}
 
-  // ---- fresh barrier state for the new group ------------------------------------------------------
+// Step 4: fresh barrier state for the new group, then every member checks every peer mapping.
+int reset_barrier(tok_comm* c, Star& star, const std::vector<Hello>& table) {
   RT_CHECK(cudaMemset(reinterpret_cast<void*>(c->local_va), 0, kFlagBytes));
   RT_CHECK(cudaMemset(c->ctr, 0, kCtrWords * sizeof(uint32_t)));
   RT_CHECK(cudaDeviceSynchronize());
@@ -835,29 +791,43 @@ int exchange(tok_comm* c) {
   RT_CHECK(cudaMemcpy(reinterpret_cast<char*>(c->local_va) + kTokenOff, &c->uid, sizeof(c->uid),
                       cudaMemcpyHostToDevice));
   RT_CHECK(cudaDeviceSynchronize());
-  if (c->world > 1) {
-    int all_reset = 0;
-    rc = star.all_ok(1, &all_reset);
-    if (rc != TOK_OK) return rc;
-    int good = 1;
-    for (int r = 0; r < c->world; ++r) {
-      uint64_t seen = 0;
-      if (cudaMemcpy(&seen, c->peer[r] + kTokenOff, sizeof(seen), cudaMemcpyDeviceToHost) != cudaSuccess ||
-          seen != table[r].uid) {
-        set_error("peer mapping check failed: rank %d's heap as mapped by rank %d carries token %llx, "
-                  "the membership table says %llx",
-                  r, c->rank, (unsigned long long)seen, (unsigned long long)table[r].uid);
-        cudaGetLastError();
-        good = 0;
-      }
+  if (c->world == 1) return TOK_OK;
+  int all_reset = 0;
+  int rc = star.all_ok(1, &all_reset);
+  if (rc != TOK_OK) return rc;
+  int good = 1;
+  for (int r = 0; r < c->world; ++r) {
+    uint64_t seen = 0;
+    if (cudaMemcpy(&seen, c->peer[r] + kTokenOff, sizeof(seen), cudaMemcpyDeviceToHost) != cudaSuccess ||
+        seen != table[r].uid) {
+      set_error("peer mapping check failed: rank %d's heap as mapped by rank %d carries token %llx, "
+                "the membership table says %llx",
+                r, c->rank, (unsigned long long)seen, (unsigned long long)table[r].uid);
+      cudaGetLastError();
+      good = 0;
     }
-    int all_good = 0;
-    rc = star.all_ok(good, &all_good);
-    if (rc != TOK_OK) return rc;
-    if (!good) return TOK_ERR_STATE;
-    if (!all_good) return fail(TOK_ERR_STATE, "a peer's mapping check failed");
   }
+  int all_good = 0;
+  rc = star.all_ok(good, &all_good);
+  if (rc != TOK_OK) return rc;
+  if (!good) return TOK_ERR_STATE;
+  if (!all_good) return fail(TOK_ERR_STATE, "a peer's mapping check failed");
   return TOK_OK;
+}
+
+// One membership exchange.  Every replica of the group runs the same steps in the same order, so
+// the socket messages and agreement rounds of each step meet their counterparts on the peers.
+// membership_dirty tells tok_comm_reform whether the old peer table survived a failure.
+int exchange(tok_comm* c) {
+  c->membership_dirty = false;
+  Star star;
+  std::vector<Hello> table(c->world);
+  std::vector<Fd> fds;
+  int rc = rendezvous(c, star, table, fds);
+  if (rc == TOK_OK) rc = rebuild_peers(c, star, table, std::move(fds));
+  if (rc == TOK_OK) rc = bind_multicast(c, star, table);
+  if (rc == TOK_OK) rc = reset_barrier(c, star, table);
+  return rc;
 }
 
 int create_impl(const char* job_id, int rank, int world, int max_world, int device_ordinal,
@@ -1061,17 +1031,9 @@ int tok_comm_destroy(tok_comm_t* c) {
     DeviceGuard guard(c->device);
     cudaDeviceSynchronize();
     teardown_multicast(c);
-    for (PeerMap& m : c->cache) {
-      if (m.own) {
-        if (m.va) {
-          drv().cuMemUnmap_(m.va, c->heap_bytes);
-          drv().cuMemAddressFree_(m.va, c->heap_bytes);
-        }
-      } else {
-        unmap_heap(c, m);
-      }
-    }
+    for (PeerMap& m : c->cache) release_peer(c, m);
     c->cache.clear();
+    unmap(c, &c->local_va);
     if (c->local_handle) drv().cuMemRelease_(c->local_handle);
     if (c->ctr) cudaFree(c->ctr);
     if (c->dbg) cudaFree(c->dbg);
