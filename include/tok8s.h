@@ -63,7 +63,7 @@ enum {
   TOK_ALGO_TWO_SHOT = 3, /* reduce-scatter + all-gather over peer HBM, two barriers              */
   TOK_ALGO_NVLS = 4,     /* NVSwitch multicast: multimem.ld_reduce + multimem.st                 */
   TOK_ALGO_LOCAL_TMA = 7 /* world == 1, one dtype: LOCAL with cp.async.bulk (TMA) through a
-                            shared-memory ring instead of LDG/STG (TOK_LOCAL_TMA=1 makes AUTO pick it) */
+                            shared-memory ring instead of LDG/STG (AUTO picks it from 1 MiB)      */
 };
 
 /* flags for tok_allreduce_bucket */

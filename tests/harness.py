@@ -8,6 +8,7 @@ the result bit-for-bit with oracle/allreduce_oracle.py.
 """
 from __future__ import annotations
 
+import math
 import multiprocessing as mp
 import os
 import sys
@@ -334,18 +335,68 @@ def _guards_intact(full, guard, count) -> bool:
     return bool((b[:guard * es] == GUARD_BYTE).all() and (b[(guard + count) * es:] == GUARD_BYTE).all())
 
 
+def expected_kernel(b: dict, world: int, multicast: bool, elide: bool = True):
+    """Restatement of the kernel plan_allreduce (csrc/plan.cpp) picks for bucket `b`: 'elided', the
+    kernel's name, or the error code the planner refuses the call with.
+
+    b holds dtype, wire, wire_bytes, in_pool and algo_for (tok_allreduce_algo's answer for
+    wire_bytes, so TOK_ALGO is in it); optionally out (default dtype), scale (default 1/world), post,
+    algo (forced through the call's flags, default AUTO), no_zero_copy, in_place (default True) and
+    zero_copy (the communicator's, default True).  elide=False stands for TOK_FLAG_NO_ELIDE."""
+    from torch_on_k8s_b200._ffi import ALGO_NAMES, TOK_ERR_INVALID, TOK_ERR_UNSUPPORTED
+    din, dw, dout = b["dtype"], b["wire"], b.get("out", b["dtype"])
+    same = din == dw == dout
+    scale = float(np.float32(b.get("scale", 1.0 / world)))
+    post = b.get("post", False)
+    pow2 = scale > 0 and math.frexp(scale)[0] == 0.5
+    forced = b.get("algo", 0)
+    algo = forced or b["algo_for"]
+    if not forced and algo == 4 and post and dw != "f32" and (dw == "f16" or not pow2):
+        algo = 3     # the switch would round the sum before a POST scale rounds it again
+    if algo == 7:
+        if world != 1 or not same:
+            return TOK_ERR_INVALID
+    elif algo not in (1, 2, 3, 4):
+        return TOK_ERR_INVALID
+    if algo in (1, 7) and world != 1:
+        return TOK_ERR_INVALID
+    if algo == 4 and not multicast:
+        return TOK_ERR_UNSUPPORTED
+    in_place = b.get("in_place", True)
+    if world == 1:
+        if not forced and in_place and same and scale == 1.0 and elide:
+            return "elided"
+        if algo == 1 and not forced and same and b["wire_bytes"] >= (1 << 20):
+            algo = 7
+        return ALGO_NAMES[algo]
+    pool_ok = (b.get("zero_copy", True) and not b.get("no_zero_copy", False) and in_place and same
+               and b["in_pool"] and b["wire_bytes"] % 16 == 0)
+    if not forced and algo == 2 and pool_ok and world == 2 and b["wire_bytes"] >= (8 << 20):
+        algo = 3     # the in-place exchange needs no staging pass
+    if pool_ok and algo in (3, 4):
+        nvls_exact = (post or pow2) and (dw != "f16" or post)
+        if algo == 4 and not nvls_exact:
+            return "nvls" if forced else "two_shot_inplace"
+        return "nvls_inplace" if algo == 4 else "two_shot_inplace"
+    return ALGO_NAMES[algo]
+
+
 def plan_launches(count: int, din: str, dw: str, dout: str, world: int, algo: int, *,
                   inplace: bool = False, staging_mb: int = 32, max_ctas: int = 16,
-                  cta_bytes: int = 65536) -> List[dict]:
-    """Restatement of how tok_allreduce_bucket splits a staged (algo 2 one-shot, 3 two-shot) or
-    zero-copy (inplace) bucket into launches and sizes each grid (csrc/comm.cpp): per launch the
-    element count n, total_packs, the slab length L (packs per CTA), the sub-slab M = L / world and
-    the grid size.  max_ctas stands for TOK_MAX_CTAS, which also caps the zero-copy grid when set."""
+                  cta_bytes: int = 65536, zc_ctas: Optional[int] = None,
+                  sm_count: int = 132) -> List[dict]:
+    """Restatement of how tok_allreduce_bucket splits a bucket into launches and sizes each grid
+    (plan_allreduce / allreduce_grid, csrc/plan.cpp): per launch the element count n, total_packs,
+    the slab length L (packs per CTA), the sub-slab M = L / world and the grid size.  algo is the
+    kernel: 1 the LDG.128 wave, 7 the TMA ring (world 1, one launch), 2 one-shot, 3 two-shot, 4 NVLS
+    (staged, or zero-copy with inplace).  max_ctas stands for TOK_MAX_CTAS; zc_ctas for TOK_ZC_CTAS,
+    0 meaning unset with TOK_MAX_CTAS unset too, and None (the default) for TOK_MAX_CTAS set, which
+    then caps the zero-copy grid as well."""
     P = 4 if "f32" in (din, dw, dout) else 8
     wsz = 4 if dw == "f32" else 2
     cap_bytes = -(-(staging_mb << 20) // (2 << 20)) * (2 << 20)
-    if inplace:
-        launch_cap = count
+    if inplace or algo in (1, 7):
+        launch_cap = 1 << 40
     else:
         launch_cap = (cap_bytes // 8 if algo == 2 else cap_bytes) // wsz
         launch_cap = launch_cap // (P * 8) * (P * 8)
@@ -353,11 +404,43 @@ def plan_launches(count: int, din: str, dw: str, dout: str, world: int, algo: in
     for off in range(0, count, launch_cap):
         n = min(launch_cap, count - off)
         packs = -(-n // P)
-        g = min(max(-(-(packs * P * wsz) // cta_bytes), 1), max_ctas)
+        if algo == 1:      # one even wave, at most 2 CTAs per SM, >= 8 packs per thread
+            full = n // P
+            g = min(max(-(-full // (512 * 8)), 1), 2 * sm_count)
+            out.append(dict(n=n, packs=packs, L=-(-max(full, 1) // g), ctas=g, P=P))
+            continue
+        if algo == 7:      # one 16 KiB tile per CTA
+            g = min(max(-(-(n // P * 16) // 16384), 1), 2 * sm_count)
+            out.append(dict(n=n, packs=packs, L=0, ctas=g, P=P))
+            continue
+        cap = max_ctas
+        if inplace:
+            zc = max_ctas if zc_ctas is None else zc_ctas
+            cap = zc or (16 if algo == 4 and packs * P * wsz >= (32 << 20) else 64)
+        g = min(max(-(-(packs * P * wsz) // cta_bytes), 1), cap)
         L = -(-packs // g)
         if algo != 2:
             L = -(-L // world) * world
         out.append(dict(n=n, packs=packs, L=L, M=L // world, ctas=-(-packs // L), P=P))
+    return out
+
+
+def bcast_launches(nbytes: int, world: int, multicast: bool, pooled: bool, *, staging_mb: int = 32,
+                   cta_bytes: int = 65536) -> List[dict]:
+    """Restatement of tok_broadcast's plan (plan_broadcast / broadcast_grid, csrc/plan.cpp): per launch
+    the kernel, the byte count n, the packs per CTA L and the grid size.  `pooled` means the buffer
+    lies in the symmetric pool and zero copy is on."""
+    if pooled and nbytes % 16 == 0:
+        kernel, chunk = ("bcast_mc_push" if multicast and world >= 3 else "bcast_pull"), nbytes
+    else:
+        kernel, chunk = "bcast_staged", -(-(staging_mb << 20) // (2 << 20)) * (2 << 20)
+    out = []
+    for off in range(0, nbytes, chunk):
+        n = min(chunk, nbytes - off)
+        packs = max(n // 16, 1)
+        g = min(max(-(-n // cta_bytes), 1), 128)
+        L = -(-packs // g)
+        out.append(dict(kernel=kernel, n=n, L=L, ctas=-(-packs // L)))
     return out
 
 

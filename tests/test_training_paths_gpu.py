@@ -255,26 +255,6 @@ def _configs(world):
     return out
 
 
-def expected_kernel(b, world, multicast, elide=True):
-    """The kernel tok_allreduce_bucket's planner (plan_bucket, csrc/comm.cpp) must take for a
-    1/world PRE bucket: 'elided', or the kernel's name."""
-    from torch_on_k8s_b200._ffi import ALGO_NAMES
-    same = b["dtype"] == b["wire"]
-    if world == 1:
-        if same and elide:
-            return "elided"
-        tma = same and b["wire_bytes"] >= (1 << 20) and os.environ.get("TOK_LOCAL_TMA", "1") != "0"
-        return "local_tma" if tma else "local"
-    algo = ALGO_NAMES[b["algo_for"]]
-    pool_ok = b["in_pool"] and same and b["wire_bytes"] % 16 == 0
-    if algo == "one_shot" and pool_ok and world == 2 and b["wire_bytes"] >= (8 << 20):
-        algo = "two_shot"
-    if pool_ok and algo in ("two_shot", "nvls"):
-        pow2 = (world & (world - 1)) == 0 and b["dtype"] != "f16"
-        return "nvls_inplace" if algo == "nvls" and multicast and pow2 else "two_shot_inplace"
-    return algo
-
-
 def oracle_close(got, want, dtype):
     """NVLS sums in the switch in an unspecified order: within the existing NVLS tolerance."""
     from oracle.allreduce_oracle import to_f32, ulp_distance
@@ -313,7 +293,7 @@ def check_ddp(res, world):
         # 2. the kernel follows the planner's rule; the arrival happened exactly for in-place buckets
         for r in ranks:
             for b in runs[r]["buckets"]:
-                want = expected_kernel(b, world, runs[r]["multicast"], elide)
+                want = harness.expected_kernel(b, world, runs[r]["multicast"], elide)
                 where = (name, r, b["step"], b["index"], b["nbytes"], b.get("in_pool"))
                 if want == "elided":
                     assert b["elided"] == 1 and b["launched"] == 0, where

@@ -760,8 +760,8 @@ __global__ void __launch_bounds__(kThreads, 2) local_kernel(const __grid_constan
 // tiles through a ring of kTmaStages shared-memory buffers: one elected thread issues
 // cp.async.bulk global->shared (completion counted in bytes on an mbarrier), all threads scale the
 // tile in shared memory, the elected thread issues cp.async.bulk shared->global and refills the
-// stage whose store has finished reading.  SASS: UBLKCP + SYNCS.  Whether this beats the LDG.128
-// wave above is a measurement (tools/local_bench.py -> profiles/); the host picks by TOK_LOCAL_TMA.
+// stage whose store has finished reading.  SASS: UBLKCP + SYNCS.  It beat the LDG.128 wave above at
+// every size measured (tools/local_bench.py), so AUTO takes it from 1 MiB; flags can force either.
 // ------------------------------------------------------------------------------------------------
 constexpr int kTmaStages = 4;
 constexpr int kTmaTileBytes = 16384;
@@ -1365,12 +1365,6 @@ int launch_broadcast(int mode, int ctas, const KArgs& args, void* stream) {
       return static_cast<int>(cudaErrorInvalidValue);
   }
   return static_cast<int>(cudaGetLastError());
-}
-
-size_t dtype_size(int dtype) { return dtype == TOK_F32 ? 4 : 2; }
-
-int pack_elems(int in_dtype, int wire_dtype, int out_dtype) {
-  return (in_dtype == TOK_F32 || wire_dtype == TOK_F32 || out_dtype == TOK_F32) ? 4 : 8;
 }
 
 int launch_allreduce(int algo, int in_dtype, int wire_dtype, int out_dtype, int ctas,

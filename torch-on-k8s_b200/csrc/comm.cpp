@@ -1,7 +1,7 @@
 // comm.cpp — replica communicator: binds one worker replica to one GPU, owns its symmetric heap
 // (CUDA VMM, exported as POSIX fds), exchanges handles with the job's other replicas over a unix
 // socket, optionally binds an NVSwitch multicast object, re-forms the group in place on elastic
-// add/drop, and plans + launches the allreduce kernels of allreduce.cu.
+// add/drop, and launches the kernels of allreduce.cu as plan.cpp decides.
 //
 // Reference side: this is what stands behind the env contract of
 // TorchJobReconciler.SetClusterSpec (controllers/train/torchjob_controller.go:394-446):
@@ -12,7 +12,6 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <errno.h>
-#include <math.h>
 #include <fcntl.h>
 #include <poll.h>
 #include <stdarg.h>
@@ -34,7 +33,7 @@
 #include <string>
 #include <vector>
 
-#include "tok_internal.h"
+#include "plan.h"
 
 namespace tok {
 
@@ -361,7 +360,6 @@ struct tok_comm {
   std::vector<std::pair<size_t, size_t>> pool_free;  // (offset, bytes) of released segments, by offset
   std::mutex pool_mu;      // tok_pool_malloc may be entered from any allocator-calling thread
   size_t heap_bytes = 0;
-  bool zero_copy = true;
   CUmemGenericAllocationHandle local_handle = 0;
   CUdeviceptr local_va = 0;
 
@@ -377,19 +375,7 @@ struct tok_comm {
   volatile uint32_t* hostctl = nullptr; // pinned host page
   uint32_t* hostctl_dev = nullptr;
 
-  // tunables
-  int max_ctas = 64;
-  int zc_ctas = 0;          // 0 = built-in rule for the zero-copy kernels
-  size_t cta_bytes = 65536;
-  size_t one_shot_max = 256 << 10;
-  bool one_shot_max_env = false;
-  size_t nvls_min = 0;
-  int force_algo = 0;
-  bool disable_nvls = false;
-  unsigned long long barrier_timeout_ns = 600000ull * 1000000ull;
-  double rdzv_timeout_s = 120;
-  int local_tma = 1;        // world 1, one dtype: 1 = cp.async.bulk variant, 0 = LDG.128 wave
-  int nvls_unroll = 8;      // multimem.ld_reduce in flight per thread in the zero-copy NVLS kernel
+  Tunables tun;
 
   std::atomic<uint64_t> launches{0};    // exchange / broadcast / local kernels
   std::atomic<uint64_t> arrivals{0};    // arrive kernels
@@ -483,7 +469,7 @@ int alloc_local(tok_comm* c) {
 
   int mc = 0;
   d.cuDeviceGetAttribute_(&mc, CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED, c->cu_dev);
-  c->mc_supported = (mc && !c->disable_nvls) ? 1 : 0;
+  c->mc_supported = (mc && !c->tun.disable_nvls) ? 1 : 0;
   size_t total = kFlagBytes + 2 * c->cap_bytes + c->pool_bytes;
   if (c->mc_supported && c->max_world > 1) {
     CUmulticastObjectProp mp;
@@ -528,7 +514,7 @@ int alloc_local(tok_comm* c) {
 int rendezvous(tok_comm* c, Star& star, std::vector<Hello>& table, std::vector<Fd>& fds) {
   star.root = (c->rank == 0);
   star.world = c->world;
-  star.deadline = now_s() + c->rdzv_timeout_s;
+  star.deadline = now_s() + c->tun.rdzv_timeout_s;
   char suffix[32];
   snprintf(suffix, sizeof(suffix), ".e%llu", static_cast<unsigned long long>(c->epoch));
   star.path = c->rdzv_path + suffix;
@@ -591,7 +577,7 @@ int rendezvous(tok_comm* c, Star& star, std::vector<Hello>& table, std::vector<F
       if (wait_fd(star.listen_fd, POLLIN, star.deadline) <= 0)
         return fail(TOK_ERR_RENDEZVOUS,
                     "rendezvous %s: only %d of %d replicas joined within %.0f s", star.path.c_str(),
-                    joined, c->world, c->rdzv_timeout_s);
+                    joined, c->world, c->tun.rdzv_timeout_s);
       int s = accept4(star.listen_fd, nullptr, nullptr, SOCK_CLOEXEC);
       if (s < 0) {
         --joined;
@@ -636,7 +622,7 @@ int rendezvous(tok_comm* c, Star& star, std::vector<Hello>& table, std::vector<F
       close(s);
       if (now_s() > star.deadline)
         return fail(TOK_ERR_RENDEZVOUS, "rendezvous %s: the group root never appeared (%.0f s)",
-                    star.path.c_str(), c->rdzv_timeout_s);
+                    star.path.c_str(), c->tun.rdzv_timeout_s);
       usleep(20000);
     }
     star.conn.assign(1, s);
@@ -830,6 +816,24 @@ int exchange(tok_comm* c) {
   return rc;
 }
 
+Tunables read_tunables() {
+  Tunables t;
+  t.zero_copy = env_size("TOK_DISABLE_ZERO_COPY", 0) == 0;
+  t.max_ctas = static_cast<int>(std::clamp<size_t>(env_size("TOK_MAX_CTAS", 64), 1, kMaxCtas));
+  t.zc_ctas = static_cast<int>(std::min<size_t>(env_size("TOK_ZC_CTAS", getenv("TOK_MAX_CTAS") ? t.max_ctas : 0), kMaxCtas));
+  t.cta_bytes = std::max<size_t>(env_size("TOK_CTA_BYTES", 65536), 4096);
+  if (getenv("TOK_ONE_SHOT_MAX")) t.one_shot_max = env_size("TOK_ONE_SHOT_MAX", 256 << 10);
+  t.nvls_min = env_size("TOK_NVLS_MIN", 0);
+  t.force_algo = static_cast<int>(env_size("TOK_ALGO", 0));
+  t.disable_nvls = env_size("TOK_DISABLE_NVLS", 0) != 0;
+  // NCCL's watchdog default is 600 s; replicas legitimately skew by tens of seconds (first-iteration
+  // cuDNN autotune, evaluation or a checkpoint on rank 0)
+  t.barrier_timeout_ns = env_size("TOK_BARRIER_TIMEOUT_MS", 600000) * 1000000ull;
+  t.nvls_unroll = env_size("TOK_NVLS_UNROLL", 8) == 16 ? 16 : 8;
+  t.rdzv_timeout_s = static_cast<double>(env_size("TOK_RDZV_TIMEOUT_S", 120));
+  return t;
+}
+
 int create_impl(const char* job_id, int rank, int world, int max_world, int device_ordinal,
                 const char* rendezvous_path, uint64_t epoch, tok_comm_t** out) {
   if (!out) return fail(TOK_ERR_INVALID, "comm out pointer is null");
@@ -865,24 +869,7 @@ int create_impl(const char* job_id, int rank, int world, int max_world, int devi
   if (c->uid == 0) c->uid = 1;
   c->cap_bytes = round_up(env_size("TOK_STAGING_MB", 128) << 20, 2u << 20);
   c->pool_bytes = round_up(env_size("TOK_SYMM_POOL_MB", 1024) << 20, 2u << 20);
-  c->zero_copy = env_size("TOK_DISABLE_ZERO_COPY", 0) == 0;
-  c->max_ctas = static_cast<int>(std::min<size_t>(env_size("TOK_MAX_CTAS", 64), kMaxCtas));
-  if (c->max_ctas < 1) c->max_ctas = 1;
-  c->zc_ctas = static_cast<int>(std::min<size_t>(env_size("TOK_ZC_CTAS", getenv("TOK_MAX_CTAS") ? c->max_ctas : 0), kMaxCtas));
-  c->cta_bytes = std::max<size_t>(env_size("TOK_CTA_BYTES", 65536), 4096);
-  c->one_shot_max_env = getenv("TOK_ONE_SHOT_MAX") != nullptr;
-  c->one_shot_max = env_size("TOK_ONE_SHOT_MAX", 256 << 10);
-  c->nvls_min = env_size("TOK_NVLS_MIN", 0);
-  c->force_algo = static_cast<int>(env_size("TOK_ALGO", 0));
-  c->disable_nvls = env_size("TOK_DISABLE_NVLS", 0) != 0;
-  // NCCL's watchdog default is 600 s; replicas legitimately skew by tens of seconds (first-iteration
-  // cuDNN autotune, evaluation or a checkpoint on rank 0)
-  c->barrier_timeout_ns = env_size("TOK_BARRIER_TIMEOUT_MS", 600000) * 1000000ull;
-  // the cp.async.bulk ring is the default for same-dtype buckets from 1 MiB (tools/local_bench.py
-  // compares it with the LDG.128 wave; DESIGN.md §6 has the H100 numbers)
-  c->local_tma = static_cast<int>(env_size("TOK_LOCAL_TMA", 1));
-  c->nvls_unroll = env_size("TOK_NVLS_UNROLL", 8) == 16 ? 16 : 8;
-  c->rdzv_timeout_s = static_cast<double>(env_size("TOK_RDZV_TIMEOUT_S", 120));
+  c->tun = read_tunables();
 
   int rc = TOK_OK;
   do {
@@ -907,37 +894,16 @@ int create_impl(const char* job_id, int rank, int world, int max_world, int devi
   return TOK_OK;
 }
 
-// Algorithm selector.  The thresholds were tuned on an 8-GPU NVSwitch system and have not been
-// re-measured on H100 (NVLink 4, 450 GB/s per direction); the shape of the rule holds: one-shot
-// moves (N-1)*S per GPU but needs a single barrier, so it wins while the bucket is latency-bound —
-// the smaller the group, the longer; NVLS wins as soon as there are >= 3 replicas and the bucket is
-// past the one-shot range; at N == 2 the in-switch reduction saves nothing and two-shot is faster.
-size_t one_shot_limit(const tok_comm* c) {
-  if (c->one_shot_max_env) return c->one_shot_max;
-  const bool mc = c->mc_va != 0;
-  switch (c->world) {
-    case 2: return 16u << 20;
-    case 3:
-    case 4: return mc ? (2u << 20) : (8u << 20);
-    case 5:
-    case 6: return mc ? (64u << 10) : (2u << 20);
-    default: return mc ? (32u << 10) : (1u << 20);
-  }
+Group group(const tok_comm* c) { return {c->world, c->mc_va != 0, c->cap_bytes, c->sm_count}; }
+
+// Start of the symmetric pool in this replica's heap: after the control page and both staging buffers.
+char* pool_base(const tok_comm* c) {
+  return reinterpret_cast<char*>(c->local_va) + kFlagBytes + 2 * c->cap_bytes;
 }
 
-int pick_algo(const tok_comm* c, size_t wire_bytes) {
-  if (c->world == 1) return TOK_ALGO_LOCAL;
-  if (c->force_algo >= TOK_ALGO_ONE_SHOT && c->force_algo <= TOK_ALGO_NVLS) {
-    if (c->force_algo == TOK_ALGO_NVLS && !c->mc_va) return TOK_ALGO_TWO_SHOT;
-    return c->force_algo;
-  }
-  const size_t slot = c->cap_bytes / kMaxWorld;
-  if (wire_bytes <= one_shot_limit(c) && wire_bytes <= slot) return TOK_ALGO_ONE_SHOT;
-  // staged path: with 3-4 replicas the in-switch reduction stops paying off past ~12 MiB (two-shot
-  // beat NVLS at 16 MiB, N=4, in the tuning sweeps); zero-copy buckets re-promote to NVLS
-  const bool nvls_ok = c->mc_va && c->world >= 3 && wire_bytes >= c->nvls_min;
-  if (nvls_ok && (c->world >= 5 || wire_bytes < (12u << 20))) return TOK_ALGO_NVLS;
-  return TOK_ALGO_TWO_SHOT;
+bool in_pool(const tok_comm* c, const void* p, size_t bytes) {
+  const char* q = static_cast<const char*>(p);
+  return q >= pool_base(c) && q + bytes <= pool_base(c) + c->pool_bytes;
 }
 
 }  // namespace
@@ -1009,7 +975,7 @@ int tok_comm_status(tok_comm_t* c) {
     return fail(TOK_ERR_TIMEOUT,
                 "a peer replica never reached the in-kernel barrier within %llu ms (rank %d of %d; "
                 "given up in %s, CTA %u, ranks still behind: mask 0x%x, waited for value %u)",
-                c->barrier_timeout_ns / 1000000ull, c->rank, c->world,
+                c->tun.barrier_timeout_ns / 1000000ull, c->rank, c->world,
                 (where & 0xff) == 1 ? "the bucket arrival" : (where & 0xff) == 2 ? "a CTA barrier" : "?",
                 where >> 8, c->hostctl[kCtlBehind], c->hostctl[kCtlWant]);
   }
@@ -1057,16 +1023,16 @@ int tok_comm_caps(tok_comm_t* c, tok_caps_t* caps) {
   caps->epoch = c->epoch;
   caps->staging_bytes = c->cap_bytes;
   caps->heap_bytes = c->heap_bytes;
-  caps->one_shot_max = one_shot_limit(c);
-  caps->nvls_min = c->nvls_min;
-  caps->max_ctas = c->max_ctas;
+  caps->one_shot_max = one_shot_limit(group(c), c->tun);
+  caps->nvls_min = c->tun.nvls_min;
+  caps->max_ctas = c->tun.max_ctas;
   caps->sm_count = c->sm_count;
   return TOK_OK;
 }
 
 int tok_allreduce_algo(tok_comm_t* c, size_t wire_bytes, int* algo) {
   if (!c || !algo) return fail(TOK_ERR_INVALID, "comm / algo is null");
-  *algo = pick_algo(c, wire_bytes);
+  *algo = pick_algo(group(c), c->tun, wire_bytes);
   return TOK_OK;
 }
 
@@ -1074,13 +1040,11 @@ int tok_allreduce_algo(tok_comm_t* c, size_t wire_bytes, int* algo) {
 // First-fit over the released segments (lowest offset first), else bump.  Deterministic: replicas
 // that perform the same allocate/release sequence get the same offsets — which is all the zero-copy
 // path needs, and the arrive kernel verifies it for every bucket.
-static size_t pool_base_off(const tok_comm* c) { return kFlagBytes + 2 * c->cap_bytes; }
-
 int tok_comm_symm_alloc(tok_comm_t* c, size_t bytes, void** ptr) {
   if (!c || !ptr) return fail(TOK_ERR_INVALID, "comm / ptr is null");
   const size_t need = round_up(std::max<size_t>(bytes, 1), 2u << 20);  // segment-friendly alignment
   std::lock_guard<std::mutex> lock(c->pool_mu);
-  char* base = reinterpret_cast<char*>(c->local_va) + pool_base_off(c);
+  char* base = pool_base(c);
   for (size_t i = 0; i < c->pool_free.size(); ++i) {
     auto& blk = c->pool_free[i];
     if (blk.second < need) continue;
@@ -1107,7 +1071,7 @@ int tok_comm_symm_free(tok_comm_t* c, void* ptr, size_t bytes) {
   if (!ptr) return TOK_OK;
   const size_t size = round_up(std::max<size_t>(bytes, 1), 2u << 20);
   std::lock_guard<std::mutex> lock(c->pool_mu);
-  const char* base = reinterpret_cast<const char*>(c->local_va) + pool_base_off(c);
+  const char* base = pool_base(c);
   const char* p = static_cast<const char*>(ptr);
   if (p < base || p + size > base + c->pool_used || ((p - base) & ((2u << 20) - 1)))
     return fail(TOK_ERR_INVALID, "pointer %p (+%zu) is not a live symmetric-pool segment", ptr, size);
@@ -1134,7 +1098,7 @@ int tok_comm_symm_free(tok_comm_t* c, void* ptr, size_t bytes) {
 
 int tok_comm_symm_info(tok_comm_t* c, void** base, size_t* bytes, size_t* used) {
   if (!c) return fail(TOK_ERR_INVALID, "comm is null");
-  if (base) *base = reinterpret_cast<char*>(c->local_va) + pool_base_off(c);
+  if (base) *base = pool_base(c);
   if (bytes) *bytes = c->pool_bytes;
   if (used) {
     std::lock_guard<std::mutex> lock(c->pool_mu);
@@ -1199,21 +1163,9 @@ int tok_comm_stats(tok_comm_t* c, tok_stats_t* st) {
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------------
-// planning: which kernel a bucket takes
+// executing plan.cpp's plans
 // ------------------------------------------------------------------------------------------------
 namespace {
-
-bool is_pow2_scale(float s) {
-  int e = 0;
-  return s > 0.f && frexpf(s, &e) == 0.5f;
-}
-
-struct Plan {
-  int algo = 0;          // TOK_ALGO_* or an internal id
-  bool inplace = false;  // zero-copy (preceded by an arrival)
-  size_t buf_off = 0;
-  bool elide = false;
-};
 
 void fill_common(const tok_comm* c, KArgs* a) {
   memset(a, 0, sizeof(*a));
@@ -1224,97 +1176,21 @@ void fill_common(const tok_comm* c, KArgs* a) {
   a->mc = reinterpret_cast<char*>(c->mc_va);
   a->ctr = c->ctr;
   a->hostctl = c->hostctl_dev;
-  a->timeout_ns = c->barrier_timeout_ns;
+  a->timeout_ns = c->tun.barrier_timeout_ns;
   a->dbg = c->dbg;
   a->rank = c->rank;
   a->world = c->world;
-  a->unroll = c->nvls_unroll;
+  a->unroll = c->tun.nvls_unroll;
 }
 
-bool in_pool(const tok_comm* c, const void* p, size_t bytes) {
-  const char* lo = reinterpret_cast<const char*>(c->local_va) + kFlagBytes + 2 * c->cap_bytes;
-  const char* q = static_cast<const char*>(p);
-  return q >= lo && q + bytes <= lo + c->pool_bytes;
+size_t heap_off(const tok_comm* c, const void* p) {
+  return static_cast<size_t>(static_cast<const char*>(p) - reinterpret_cast<const char*>(c->local_va));
 }
 
-int plan_bucket(const tok_comm* c, const void* in, const void* out, size_t count, int in_dtype,
-                int wire_dtype, int out_dtype, float scale, unsigned flags, Plan* pl) {
-  const size_t wsz = dtype_size(wire_dtype);
-  const size_t isz = dtype_size(in_dtype);
-  const bool same_dt = in_dtype == wire_dtype && wire_dtype == out_dtype;
-  int algo = static_cast<int>((flags & TOK_FLAG_ALGO_MASK) >> TOK_FLAG_ALGO_SHIFT);
-  const bool forced = algo != TOK_ALGO_AUTO;
-  const bool post = (flags & TOK_FLAG_SCALE_POST) != 0;
-  if (algo == TOK_ALGO_AUTO) algo = pick_algo(c, count * wsz);
-  // The switch returns the sum already rounded to the wire dtype, so a POST scale rounds a second
-  // time: exact for a power-of-two factor on a bf16 wire, 1 ulp off for other factors, and an f16
-  // sum can overflow before the factor brings it back into range.  AUTO keeps such buckets on the
-  // P2P kernels, which round once (staged: two-shot; pool buckets: two-shot in place, below).
-  // `forced` is an algorithm in the call's flags; TOK_ALGO in the environment only replaces
-  // pick_algo's choice by size and stays under this rule, as under the pool-bucket rule below.
-  if (!forced && algo == TOK_ALGO_NVLS && post && wire_dtype != TOK_F32 &&
-      (wire_dtype == TOK_F16 || !is_pow2_scale(scale)))
-    algo = TOK_ALGO_TWO_SHOT;
-  if (algo == TOK_ALGO_LOCAL_TMA) {
-    if (c->world != 1 || !same_dt)
-      return fail(TOK_ERR_INVALID, "TOK_ALGO_LOCAL_TMA needs world == 1 and one dtype");
-    algo = kAlgoLocalTma;
-  } else if (algo < TOK_ALGO_LOCAL || algo > TOK_ALGO_NVLS) {
-    return fail(TOK_ERR_INVALID, "unknown algorithm %d", algo);
-  }
-  if ((algo == TOK_ALGO_LOCAL || algo == kAlgoLocalTma) && c->world != 1)
-    return fail(TOK_ERR_INVALID, "TOK_ALGO_LOCAL is only valid for world == 1 (world is %d)",
-                c->world);
-  if (algo == TOK_ALGO_NVLS && !c->mc_va)
-    return fail(TOK_ERR_UNSUPPORTED,
-                "NVLS requested but no multicast object is bound for this group");
-  if (c->world == 1) {
-    // a bucket that is already what the caller asked for needs no pass over HBM at all
-    pl->elide = !forced && in == out && same_dt && scale == 1.0f && !(flags & TOK_FLAG_NO_ELIDE);
-    if (algo == TOK_ALGO_LOCAL && !forced && same_dt && c->local_tma &&
-        count * wsz >= (1u << 20))
-      algo = kAlgoLocalTma;
-    pl->algo = algo;
-    return TOK_OK;
-  }
-  // Zero-copy: the bucket lives in the symmetric pool (same offset on every replica), is exchanged
-  // in place, in its own dtype, in whole 16-byte packs -> peers read / multicast it directly.
-  const bool pool_ok = c->zero_copy && !(flags & TOK_FLAG_NO_ZERO_COPY) && in == out && same_dt &&
-                       in_pool(c, in, count * isz) && (count * wsz) % 16 == 0;
-  // a pool bucket leaves the one-shot range earlier: its exchange needs no staging pass (in the N=2
-  // tuning sweeps the in-place exchange caught up with one-shot at 8 MiB and beat it at 16 MiB)
-  if (!forced && algo == TOK_ALGO_ONE_SHOT && pool_ok && c->world == 2 && count * wsz >= (8u << 20))
-    algo = TOK_ALGO_TWO_SHOT;
-  bool inplace = pool_ok && (algo == TOK_ALGO_TWO_SHOT || algo == TOK_ALGO_NVLS);
-  if (inplace) {
-    // The switch can only scale the SUM.  That equals the specified PRE semantics (scale every
-    // contribution, then sum) when the factor is a power of two; a 16-bit float sum may also
-    // overflow before the 1/N is applied.  POST buckets that reach this point are either forced or
-    // passed the rule above.  Everything else takes the P2P in-place kernel, which applies PRE
-    // exactly as the staged path does.
-    const bool nvls_exact = (post || is_pow2_scale(scale)) && (wire_dtype != TOK_F16 || post);
-    // (pick_algo's rule stands for pool buckets too: with 3-4 replicas the in-switch reduction stops
-    // paying off past ~12 MiB — P2P reduce+push beat NVLS in place at N=4 on the 22.9 / 28.3 MB DDP
-    // buckets in the tuning sweeps; with >= 5 replicas NVLS won)
-    if (algo == TOK_ALGO_NVLS && !nvls_exact) {
-      if (forced)
-        inplace = false;  // honour the forced algorithm through the staged kernel
-      else
-        algo = TOK_ALGO_TWO_SHOT;
-    }
-  }
-  if (inplace) {
-    pl->buf_off = static_cast<size_t>(static_cast<const char*>(in) -
-                                      reinterpret_cast<const char*>(c->local_va));
-    algo = (algo == TOK_ALGO_NVLS) ? kAlgoNvlsInplace : kAlgoTwoShotInplace;
-  }
-  pl->inplace = inplace;
-  pl->algo = algo;
-  return TOK_OK;
-}
-
-int check_bucket_args(tok_comm* c, const void* in, const void* out, int in_dtype, int wire_dtype,
-                      int out_dtype) {
+// Checks a bucket call's arguments and the group's health, then plans the bucket.
+int plan_bucket(tok_comm* c, const void* in, const void* out, size_t count, int in_dtype,
+                int wire_dtype, int out_dtype, float scale, unsigned flags, Bucket* b,
+                AllreducePlan* pl) {
   if (!c) return fail(TOK_ERR_INVALID, "comm is null");
   auto bad_dt = [](int d) { return d != TOK_F32 && d != TOK_BF16 && d != TOK_F16; };
   if (bad_dt(in_dtype) || bad_dt(wire_dtype) || bad_dt(out_dtype))
@@ -1323,7 +1199,16 @@ int check_bucket_args(tok_comm* c, const void* in, const void* out, int in_dtype
   if (!in || !out) return fail(TOK_ERR_INVALID, "in / out is null");
   if ((reinterpret_cast<uintptr_t>(in) & 15) || (reinterpret_cast<uintptr_t>(out) & 15))
     return fail(TOK_ERR_ALIGN, "bucket pointers must be 16-byte aligned (in %p out %p)", in, out);
-  return tok_comm_status(c);
+  const int st = tok_comm_status(c);
+  if (st != TOK_OK) return st;
+  *b = {count, in_dtype, wire_dtype, out_dtype, scale, flags, in == out,
+        in_pool(c, in, count * dtype_size(in_dtype))};
+  return plan_allreduce(group(c), c->tun, *b, pl);
+}
+
+int launch_error(const char* what, int e) {
+  return fail(TOK_ERR_CUDA, "%s launch failed: %s", what,
+              cudaGetErrorString(static_cast<cudaError_t>(e)));
 }
 
 int do_arrive(tok_comm* c, size_t buf_off, void* stream) {
@@ -1331,10 +1216,17 @@ int do_arrive(tok_comm* c, size_t buf_off, void* stream) {
   fill_common(c, &a);
   a.buf_off = buf_off;
   int e = launch_arrive(a, stream);
-  if (e != 0)
-    return fail(TOK_ERR_CUDA, "arrive kernel launch failed: %s",
-                cudaGetErrorString(static_cast<cudaError_t>(e)));
+  if (e != 0) return launch_error("arrive kernel", e);
   c->arrivals.fetch_add(1);
+  return TOK_OK;
+}
+
+// Takes the result `e` of launching a `what` kernel: counts the launch, or reports its error.
+int launched(tok_comm* c, int e, const char* what, int algo, int ctas) {
+  if (e != 0) return launch_error(what, e);
+  c->launches.fetch_add(1);
+  c->last_algo.store(algo);
+  c->last_ctas.store(ctas);
   return TOK_OK;
 }
 
@@ -1346,14 +1238,13 @@ int tok_bucket_arrive(tok_comm_t* c, const void* bucket, size_t count, int dtype
                       unsigned flags, void* cuda_stream, int* arrived) {
   if (arrived) *arrived = 0;
   if (count == 0) return TOK_OK;
-  int st = check_bucket_args(c, bucket, bucket, dtype, dtype, dtype);
-  if (st != TOK_OK) return st;
-  Plan pl;
-  st = plan_bucket(c, bucket, bucket, count, dtype, dtype, dtype, scale, flags, &pl);
+  Bucket b;
+  AllreducePlan pl;
+  int st = plan_bucket(c, bucket, bucket, count, dtype, dtype, dtype, scale, flags, &b, &pl);
   if (st != TOK_OK) return st;
   if (!pl.inplace) return TOK_OK;  // staged kernels carry their own barriers
   DeviceGuard guard(c->device);
-  st = do_arrive(c, pl.buf_off, cuda_stream);
+  st = do_arrive(c, heap_off(c, bucket), cuda_stream);
   if (st == TOK_OK && arrived) *arrived = 1;
   return st;
 }
@@ -1362,88 +1253,37 @@ int tok_allreduce_bucket(tok_comm_t* c, const void* in, void* out, size_t count,
                          int wire_dtype, int out_dtype, float scale, unsigned flags,
                          void* cuda_stream) {
   if (c && count == 0) return TOK_OK;
-  int st = check_bucket_args(c, in, out, in_dtype, wire_dtype, out_dtype);
-  if (st != TOK_OK) return st;
-  Plan pl;
-  st = plan_bucket(c, in, out, count, in_dtype, wire_dtype, out_dtype, scale, flags, &pl);
+  Bucket b;
+  AllreducePlan pl;
+  int st = plan_bucket(c, in, out, count, in_dtype, wire_dtype, out_dtype, scale, flags, &b, &pl);
   if (st != TOK_OK) return st;
   if (pl.elide) {
     c->elided.fetch_add(1);
     return TOK_OK;
   }
-  const int algo = pl.algo;
-  const bool inplace = pl.inplace;
-  const int P = pack_elems(in_dtype, wire_dtype, out_dtype);
-  const size_t wsz = dtype_size(wire_dtype);
   const size_t isz = dtype_size(in_dtype);
   const size_t osz = dtype_size(out_dtype);
-  const bool local = algo == TOK_ALGO_LOCAL || algo == kAlgoLocalTma;
-
-  // largest element count one launch may take (multiple of 8 elements -> 16-byte aligned chunks)
-  size_t launch_cap = c->cap_bytes / wsz;
-  if (algo == TOK_ALGO_ONE_SHOT) launch_cap = (c->cap_bytes / kMaxWorld) / wsz;
-  launch_cap = launch_cap / (static_cast<size_t>(P) * kMaxWorld) * (static_cast<size_t>(P) * kMaxWorld);
-  if (local || inplace) launch_cap = (static_cast<size_t>(1) << 40);
-
   DeviceGuard guard(c->device);
-  if (inplace && !(flags & TOK_FLAG_ARRIVED)) {
-    st = do_arrive(c, pl.buf_off, cuda_stream);
+  if (pl.inplace && !(flags & TOK_FLAG_ARRIVED)) {
+    st = do_arrive(c, heap_off(c, in), cuda_stream);
     if (st != TOK_OK) return st;
   }
   KArgs a;
   fill_common(c, &a);
-  a.buf_off = pl.buf_off;
   a.scale = scale;
   a.flags = flags & TOK_FLAG_SCALE_POST;
-
-  for (size_t off = 0; off < count; off += launch_cap) {
-    const size_t n = std::min(launch_cap, count - off);
+  for (size_t off = 0; off < count; off += pl.launch_elems) {
+    const size_t n = std::min(pl.launch_elems, count - off);
+    const Grid grid = allreduce_grid(group(c), c->tun, b, pl, n);
     a.in = static_cast<const char*>(in) + off * isz;
     a.out = static_cast<char*>(out) + off * osz;
     a.count = n;
-    a.total_packs = (n + P - 1) / P;
-    int ctas;
-    if (algo == TOK_ALGO_LOCAL) {
-      // one even wave, at most 2 CTAs per SM, >= 8 packs per thread
-      const size_t full = n / P;
-      const size_t want = (full + kThreads * 8 - 1) / (kThreads * 8);
-      const size_t g = std::min<size_t>(std::max<size_t>(want, 1), static_cast<size_t>(c->sm_count) * 2);
-      a.packs_per_cta = (std::max<size_t>(full, 1) + g - 1) / g;
-      ctas = static_cast<int>(g);
-    } else if (algo == kAlgoLocalTma) {
-      const size_t tiles = (n / P * 16 + 16383) / 16384;
-      ctas = static_cast<int>(std::min<size_t>(std::max<size_t>(tiles, 1), static_cast<size_t>(c->sm_count) * 2));
-      a.packs_per_cta = 0;
-    } else {
-      const size_t bytes = a.total_packs * P * wsz;
-      size_t cap_ctas = c->max_ctas;
-      if (inplace) {
-        // In-place NVLS saturates the NVSwitch reduction path with few requesters: in the isolated
-        // tuning sweeps 16 CTAs beat 64 from 32 MiB up at N=8.  Below that the difference was within
-        // run-to-run noise, and the ResNet-50 buckets (22.9 / 28.3 MB) did best with 64 CTAs inside
-        // bench.py, so 64 stays the default there.  (Not re-measured on H100.)
-        if (c->zc_ctas)
-          cap_ctas = c->zc_ctas;
-        else if (algo == kAlgoNvlsInplace && bytes >= (32u << 20))
-          cap_ctas = 16;
-        else
-          cap_ctas = 64;
-      }
-      size_t g = std::min<size_t>(std::max<size_t>((bytes + c->cta_bytes - 1) / c->cta_bytes, 1),
-                                  cap_ctas);
-      size_t L = (a.total_packs + g - 1) / g;
-      if (algo != TOK_ALGO_ONE_SHOT) L = round_up(L, c->world);
-      if (inplace) a.buf_off = pl.buf_off + off * isz;
-      a.packs_per_cta = L;
-      ctas = static_cast<int>((a.total_packs + L - 1) / L);
-    }
-    int e = launch_allreduce(algo, in_dtype, wire_dtype, out_dtype, ctas, a, cuda_stream);
-    if (e != 0)
-      return fail(TOK_ERR_CUDA, "allreduce kernel launch failed: %s",
-                  cudaGetErrorString(static_cast<cudaError_t>(e)));
-    c->launches.fetch_add(1);
-    c->last_algo.store(algo);
-    c->last_ctas.store(ctas);
+    a.total_packs = grid.total_packs;
+    a.packs_per_cta = grid.packs_per_cta;
+    if (pl.inplace) a.buf_off = heap_off(c, in) + off * isz;
+    st = launched(c, launch_allreduce(pl.algo, in_dtype, wire_dtype, out_dtype, grid.ctas, a, cuda_stream),
+                  "allreduce kernel", pl.algo, grid.ctas);
+    if (st != TOK_OK) return st;
   }
   return TOK_OK;
 }
@@ -1470,10 +1310,7 @@ int tok_comm_debug_barrier(tok_comm_t* c, int variant, int ctas, size_t count, v
   a.count = count;
   a.flags = static_cast<uint32_t>(variant);
   int e = launch_barrier_bench(ctas, a, cuda_stream);
-  if (e != 0)
-    return fail(TOK_ERR_CUDA, "barrier bench launch failed: %s",
-                cudaGetErrorString(static_cast<cudaError_t>(e)));
-  return TOK_OK;
+  return e != 0 ? launch_error("barrier bench", e) : TOK_OK;
 }
 
 int tok_broadcast(tok_comm_t* c, void* buf, size_t bytes, int root, void* cuda_stream) {
@@ -1487,51 +1324,24 @@ int tok_broadcast(tok_comm_t* c, void* buf, size_t bytes, int root, void* cuda_s
   int st = tok_comm_status(c);
   if (st != TOK_OK) return st;
   DeviceGuard guard(c->device);
-  const bool pooled = c->zero_copy && in_pool(c, buf, bytes) && bytes % 16 == 0;
+  const BroadcastPlan bp = plan_broadcast(group(c), c->tun, bytes, in_pool(c, buf, bytes));
   KArgs a;
   fill_common(c, &a);
   a.root = root;
-  auto grid = [&](size_t nbytes, KArgs* k) {
-    const size_t packs = std::max<size_t>(nbytes / 16, 1);
-    const size_t g = std::min<size_t>(std::max<size_t>((nbytes + c->cta_bytes - 1) / c->cta_bytes, 1), 128);
-    k->packs_per_cta = (packs + g - 1) / g;
-    return static_cast<int>((packs + k->packs_per_cta - 1) / k->packs_per_cta);
-  };
-  if (pooled) {
-    const size_t off = static_cast<size_t>(static_cast<char*>(buf) - reinterpret_cast<char*>(c->local_va));
-    st = do_arrive(c, off, cuda_stream);
+  if (bp.mode != kBcastStaged) {  // peers read the bucket where it lies: they wait for its arrival
+    a.buf_off = heap_off(c, buf);
+    st = do_arrive(c, a.buf_off, cuda_stream);
     if (st != TOK_OK) return st;
-    a.buf_off = off;
-    a.in = buf;
-    a.out = buf;
-    a.count = bytes;
-    // one multimem.st stream feeds N-1 receivers; with a single receiver it saves nothing and a
-    // pull (the receiver's own LDG.128 over NVLink) is the faster copy
-    const int mode = (c->mc_va && c->world >= 3) ? kBcastMcPush : kBcastPull;
-    const int ctas = grid(bytes, &a);
-    int e = launch_broadcast(mode, ctas, a, cuda_stream);
-    if (e != 0)
-      return fail(TOK_ERR_CUDA, "broadcast kernel launch failed: %s",
-                  cudaGetErrorString(static_cast<cudaError_t>(e)));
-    c->launches.fetch_add(1);
-    c->last_algo.store(mode);
-    c->last_ctas.store(ctas);
-  } else {
-    const size_t cap = c->cap_bytes;  // one staging buffer per launch
-    for (size_t off = 0; off < bytes; off += cap) {
-      const size_t n = std::min(cap, bytes - off);
-      a.in = static_cast<char*>(buf) + off;
-      a.out = static_cast<char*>(buf) + off;
-      a.count = n;
-      const int ctas = grid(n, &a);
-      int e = launch_broadcast(kBcastStaged, ctas, a, cuda_stream);
-      if (e != 0)
-        return fail(TOK_ERR_CUDA, "broadcast kernel launch failed: %s",
-                    cudaGetErrorString(static_cast<cudaError_t>(e)));
-      c->launches.fetch_add(1);
-      c->last_algo.store(kBcastStaged);
-      c->last_ctas.store(ctas);
-    }
+  }
+  for (size_t off = 0; off < bytes; off += bp.launch_bytes) {
+    const size_t n = std::min(bp.launch_bytes, bytes - off);
+    const Grid grid = broadcast_grid(c->tun, n);
+    a.in = a.out = static_cast<char*>(buf) + off;
+    a.count = n;
+    a.packs_per_cta = grid.packs_per_cta;
+    st = launched(c, launch_broadcast(bp.mode, grid.ctas, a, cuda_stream), "broadcast kernel",
+                  bp.mode, grid.ctas);
+    if (st != TOK_OK) return st;
   }
   c->broadcasts.fetch_add(1);
   return TOK_OK;

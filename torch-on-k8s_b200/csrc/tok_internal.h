@@ -85,9 +85,6 @@ int launch_allreduce(int algo, int in_dtype, int wire_dtype, int out_dtype, int 
 int launch_arrive(const KArgs& args, void* stream);
 int launch_broadcast(int mode, int ctas, const KArgs& args, void* stream);
 int launch_barrier_bench(int ctas, const KArgs& args, void* stream);  // profiling aid
-// Elements per 16-byte pack for a dtype triple (4 when any dtype is f32, else 8).
-int pack_elems(int in_dtype, int wire_dtype, int out_dtype);
-size_t dtype_size(int dtype);
 // Shared memory the TMA-staged local kernel asks for (opt-in dynamic shared memory).
 size_t local_tma_smem_bytes();
 
