@@ -26,17 +26,7 @@ edp = ElasticDataParallel(model, rep.comm)
 opt = torch.optim.SGD(model.parameters(), lr=0.05, momentum=0.9)
 x, y = batch(rep.rank, 64)
 x, y = x.to(dev), y.to(dev)
-cell = torch.zeros(2, dtype=torch.int64, device=dev)
 history = []
-
-
-def hand_over(step):
-    edp.sync_params(0)
-    edp.sync_optimizer_state(opt, 0)
-    cell[0] = step
-    rep.comm.broadcast(cell, 0)
-    torch.cuda.synchronize()
-    return int(cell[0].item())
 
 
 def digest():
@@ -48,7 +38,7 @@ import time  # noqa: E402
 step = 0
 fresh = False
 if rep.comm.caps().epoch > 0:
-    step = hand_over(0)
+    step = edp.hand_over(opt, 0)
     fresh = True      # the survivors go straight from the hand-over to the training step: so do we
     history.append(dict(event="joined", step=step, world=rep.world, rank=rep.rank,
                         epoch=rep.comm.caps().epoch))
@@ -59,7 +49,7 @@ while step < steps:
         if upd[0] == "dropped":
             history.append(dict(event="dropped", step=step))
             break
-        step = hand_over(step)
+        step = edp.hand_over(opt, step)
         history.append(dict(event="reformed", step=step, world=rep.world, rank=rep.rank,
                             epoch=rep.comm.caps().epoch))
     edp.zero_grad()

@@ -191,13 +191,7 @@ def run_cases(rank: int, world: int, device: int, path: str, cases: List[dict],
     comm = Communicator(job, rank, world, device, rendezvous_path=path)
     stream = torch.cuda.Stream(device=dev)
     results = []
-    if use_mempool:
-        symm_empty = comm.symm_empty
-    else:
-        from torch_on_k8s_b200.elastic_dp import symm_tensor
-
-        def symm_empty(n, dt):
-            return symm_tensor(comm, n, dt)
+    symm_empty = comm.symm_empty if use_mempool else comm.symm_alloc
     comm._test_symm_empty = symm_empty
     caps = comm.caps()
     try:

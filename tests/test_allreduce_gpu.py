@@ -377,8 +377,7 @@ def test_dead_peer_times_out_instead_of_hanging(tok_lib, symm):
     [t.start() for t in ts]
     [t.join(120) for t in ts]
     try:
-        from torch_on_k8s_b200.elastic_dp import symm_tensor
-        x = symm_tensor(comms[0], 4096, torch.float32).fill_(1.0) if symm else \
+        x = comms[0].symm_alloc(4096, torch.float32).fill_(1.0) if symm else \
             torch.ones(4096, device="cuda")
         # (two-shot by name for the pool bucket: AUTO takes one-shot for 16 KiB)
         comms[0].allreduce_bucket(x, x, scale=0.5, algo=3 if symm else 0)   # rank 1 never calls

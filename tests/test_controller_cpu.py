@@ -177,7 +177,7 @@ def test_torchelastic_loop_scales_workers_and_publishes_membership(tok_lib, tmp_
     members = [json.loads(e[3]) for e in ctl.events if e[2] == "MembershipPublished"]
     assert members[-1] == {"epoch": 1, "world": 3, "survivor_mask": 0b11,
                            "ranks": {"el-master-0": 0, "el-worker-0": 1, "el-worker-1": 2}}
-    from torch_on_k8s_b200.worker import membership_update
+    from torch_on_k8s_b200.membership import membership_update
     assert membership_update(members[-1], "el-worker-0", 0) == (3, 1, 0b11, 1)   # survivor re-forms
     assert membership_update(members[-1], "el-worker-1", 0) == (3, 2, 0b11, 1)   # joiner's view
     assert membership_update(members[-1], "el-worker-0", 1) is None              # already there
@@ -323,20 +323,13 @@ def test_joiner_waits_for_the_membership_that_lists_it(tmp_path):
     it was started at): it waits for the first document with epoch >= its own that lists it; a
     membership that never lists it (a reverted scale-out) times out instead of joining a wrong group."""
     import threading
-    import time
-    from torch_on_k8s_b200.worker import membership_update, wait_for_membership
+    from torch_on_k8s_b200.membership import membership_update, publish, wait_for_membership
     rdzv = str(tmp_path / "tok8s-j-1")
-
-    def publish(doc, delay):
-        time.sleep(delay)
-        with open(rdzv + ".members.tmp", "w") as f:
-            json.dump(doc, f)
-        os.replace(rdzv + ".members.tmp", rdzv + ".members")
-    with open(rdzv + ".members", "w") as f:     # an older membership without the joiner
-        json.dump({"epoch": 1, "world": 2, "ranks": {"j-master-0": 0, "j-worker-0": 1}}, f)
+    # an older membership without the joiner
+    publish(rdzv, {"epoch": 1, "world": 2, "ranks": {"j-master-0": 0, "j-worker-0": 1}})
     doc3 = {"epoch": 3, "world": 3, "survivor_mask": 3,
             "ranks": {"j-master-0": 0, "j-worker-0": 1, "j-worker-1": 2}}
-    threading.Thread(target=publish, args=(doc3, 0.3), daemon=True).start()
+    threading.Timer(0.3, publish, args=(rdzv, doc3)).start()
     assert wait_for_membership(rdzv, "j-worker-1", 2, timeout_s=10) == (2, 3, 3)
     with pytest.raises(TimeoutError):
         wait_for_membership(rdzv, "j-worker-9", 2, timeout_s=0.3)

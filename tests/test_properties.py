@@ -163,7 +163,7 @@ def test_bert_base_bucket_sizes_match_survey():
     assert sum(sizes) == 218964480
 
 
-def test_elastic_dp_bucket_layout_on_cpu(monkeypatch):
+def test_elastic_dp_bucket_layout_on_cpu():
     """ElasticDataParallel's bucket layout logic, with the symmetric-pool allocation stubbed out so
     that it runs without a GPU: grads become views of the flat buckets, in Reducer order, 16-byte
     aligned; accumulating into them and zero_grad() keep them views."""
@@ -172,13 +172,12 @@ def test_elastic_dp_bucket_layout_on_cpu(monkeypatch):
     from workloads.mlp import batch, mlp
     allocs = []
 
-    def fake_symm(comm, numel, dtype):
-        t = torch.zeros(numel, dtype=dtype)
-        allocs.append(t)
-        return t
-    monkeypatch.setattr(elastic_dp, "symm_tensor", fake_symm)
+    class FakeComm:
+        def symm_alloc(self, numel, dtype):
+            allocs.append(torch.zeros(numel, dtype=dtype))
+            return allocs[-1]
     model = mlp(0)
-    edp = elastic_dp.ElasticDataParallel(model, comm=None, bucket_cap_mb=25)
+    edp = elastic_dp.ElasticDataParallel(model, comm=FakeComm(), bucket_cap_mb=25)
     assert len(edp.buckets) == 1 and edp.buckets[0] is allocs[0]
     params = list(model.parameters())[::-1]
     off = 0
@@ -193,5 +192,5 @@ def test_elastic_dp_bucket_layout_on_cpu(monkeypatch):
     assert float(edp.buckets[0].abs().sum()) == 0 and params[0].grad is not None
     # a tiny cap forces several buckets, in the Reducer's order
     model2 = mlp(0)
-    edp2 = elastic_dp.ElasticDataParallel(model2, comm=None, bucket_cap_mb=0, first_bucket_mb=0)
+    edp2 = elastic_dp.ElasticDataParallel(model2, comm=FakeComm(), bucket_cap_mb=0, first_bucket_mb=0)
     assert len(edp2.buckets) == 4

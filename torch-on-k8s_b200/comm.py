@@ -8,6 +8,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import os
+import types
 from typing import Optional
 
 import torch
@@ -177,6 +178,60 @@ class Communicator:
     def symm_empty(self, numel: int, dtype: torch.dtype) -> torch.Tensor:
         with self.symmetric():
             return torch.empty(numel, dtype=dtype, device=torch.device("cuda", self.device))
+
+    def symm_alloc(self, numel: int, dtype: torch.dtype) -> torch.Tensor:
+        """A flat tensor carved straight from the symmetric pool, outside any torch allocator:
+        replicas that allocate and release in the same order get the same offsets.  Raises TokError
+        when the pool is exhausted.  Release it with symm_free() once nothing in flight uses it."""
+        nbytes = numel * dtype.itemsize
+        ptr = C.c_void_p()
+        check(lib().tok_comm_symm_alloc(self._h, max(nbytes, 16), C.byref(ptr)))
+        raw = types.SimpleNamespace(__cuda_array_interface__={
+            "shape": (max(nbytes, 16),), "typestr": "|u1", "data": (ptr.value, False), "version": 2})
+        return torch.as_tensor(raw, device=torch.device("cuda", self.device))[:nbytes].view(dtype)
+
+    def symm_free(self, t: torch.Tensor) -> None:
+        """Give a symm_alloc() tensor's segment back to the pool."""
+        check(lib().tok_comm_symm_free(self._h, t.data_ptr(), max(t.numel() * t.element_size(), 16)))
+
+    @torch.no_grad()
+    def broadcast_coalesced(self, tensors, root: int = 0, use_pool: bool = True) -> None:
+        """Replicate `root`'s `tensors` (any dtypes, this replica's device) into every replica's, bit
+        for bit — dist._broadcast_coalesced's job (torch/nn/parallel/distributed.py:1032): per dtype,
+        packed into one flat buffer, one tok_broadcast, unpacked in place on the receivers.
+        use_pool: the flat buffer comes from the symmetric pool when it fits — the root then feeds all
+        receivers with ONE multimem.st stream through the NVSwitch — and is released again, in the
+        same order on every replica; otherwise it is a plain buffer."""
+        by_dtype = {}
+        for t in tensors:
+            by_dtype.setdefault(t.dtype, []).append(t)
+        me = self.rank
+        for dtype, ts in by_dtype.items():
+            n = sum(t.numel() for t in ts)
+            if n == 0:
+                continue
+            n_pad = (n * dtype.itemsize + 15) // 16 * 16 // dtype.itemsize
+            flat = None
+            if use_pool:
+                try:
+                    flat = self.symm_alloc(n_pad, dtype)
+                except TokError:
+                    pass
+            pooled = flat is not None
+            if not pooled:
+                flat = torch.empty(n_pad, dtype=dtype, device=ts[0].device)
+            if me == root:
+                torch.cat([t.reshape(-1) for t in ts], out=flat[:n])
+            self.broadcast(flat, root)
+            if me != root:
+                off = 0
+                for t in ts:
+                    t.copy_(flat[off:off + t.numel()].view(t.shape))
+                    off += t.numel()
+            if pooled:
+                # the segment is recycled: nothing in flight may still use it
+                torch.cuda.current_stream(flat.device).synchronize()
+                self.symm_free(flat)
 
     # ---- elastic ------------------------------------------------------------------------------
     def reform(self, new_world: int, new_rank: int, member_mask: int, epoch: int) -> None:

@@ -31,6 +31,7 @@ import time
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
 
+from . import membership
 from .coordinator import SCHEDULING_PERIOD_S, Coordinator
 from .elastic import LOOP_PERIOD_S, ElasticPolicy, parse_log_line
 from .job import TASK_ORDER, TorchJob, should_failover
@@ -331,10 +332,11 @@ class Controller:
         return mj.epoch
 
     def _publish_membership(self, mj: ManagedJob) -> bool:
-        """Membership epoch file next to the job's rendezvous socket: the in-place replacement of the
-        reference's `distributed.io/world-size` annotation + kruise container restart
-        (controllers/train/elastic_scale.go:303-397).  Replicas poll it (worker.Replica.poll_membership)
-        and call tok_comm_reform / join at the announced epoch.
+        """Membership epoch file next to the job's rendezvous socket (membership.py): the in-place
+        replacement of the reference's `distributed.io/world-size` annotation + kruise container
+        restart (controllers/train/elastic_scale.go:303-397).  Replicas poll it at step boundaries
+        (worker.Replica.poll_membership_collective) and call tok_comm_reform / join at the announced
+        epoch.
 
         Only a membership every member of which has a live process is announced: survivors that
         re-formed towards a replica that is still Pending (no free GPU) would block in the rendezvous
@@ -342,6 +344,7 @@ class Controller:
         so does the next torchelastic pass here.  Returns True when a document was written."""
         import json
         from ._ffi import TOK_MAX_WORLD
+        rdzv = self._rdzv_path(mj)
         members, mask = {}, 0
         for tt in TASK_ORDER:
             for idx in sorted(mj.replicas.get(tt, {})):
@@ -354,8 +357,7 @@ class Controller:
                 known = mj.published["ranks"] if mj.published is not None else None
                 joiner = (known is not None and spec["name"] not in known) or \
                     (known is None and r.epoch > 0)
-                if self.wait_ready and joiner and not os.path.exists(
-                        "%s.ready.%s" % (self._rdzv_path(mj), spec["name"])):
+                if self.wait_ready and joiner and not membership.is_ready(rdzv, spec["name"]):
                     return False            # still starting up: the survivors keep training
                 members[spec["name"]] = spec["rank"]
                 # a replica's rank is a function of (task type, index), so a survivor keeps its rank:
@@ -374,17 +376,16 @@ class Controller:
         mj.membership_dirty = False
         if mj.published is not None and mj.published["ranks"] == members:
             return False                    # e.g. a scale-out that was reverted before it happened
-        path = self._rdzv_path(mj) + ".members"
         doc = {"epoch": mj.epoch, "world": world, "ranks": members, "survivor_mask": mask}
-        with open(path + ".tmp", "w") as f:
-            json.dump(doc, f)
-        os.replace(path + ".tmp", path)
+        membership.publish(rdzv, doc)
         mj.published = doc
         self._event(mj.uid, "MembershipPublished", json.dumps(doc))
         return True
 
     def _rdzv_path(self, mj: ManagedJob) -> str:
-        port = mj.job.cluster_spec("master", 0)["env"][0]["value"]
+        """The job's rendezvous socket path (TOK8S_RDZV of every replica); the membership files sit
+        next to it."""
+        port = mj.job.cluster_spec("master", 0)["env"][0]["value"]   # MASTER_PORT, job-wide
         return os.path.join(self.rdzv_dir, "tok8s-%s-%s" % (mj.job.name.replace("/", "-"), port))
 
     def _start_replica(self, mj: ManagedJob, tt: str, idx: int, restarts: int = 0) -> None:
@@ -401,9 +402,7 @@ class Controller:
         if env.get("MASTER_ADDR") not in ("localhost", "127.0.0.1"):
             env["MASTER_ADDR"] = "127.0.0.1"   # single box: the master's name resolves to loopback
         env.update(TOK8S_JOB=mj.job.name, TOK8S_REPLICA=spec["name"], TOK8S_TASK_TYPE=tt,
-                   TOK8S_TASK_INDEX=str(idx), TOK8S_EPOCH=str(mj.epoch),
-                   TOK8S_RDZV=os.path.join(self.rdzv_dir, "tok8s-%s-%s" %
-                                           (mj.job.name.replace("/", "-"), env["MASTER_PORT"])))
+                   TOK8S_TASK_INDEX=str(idx), TOK8S_EPOCH=str(mj.epoch), TOK8S_RDZV=self._rdzv_path(mj))
         if gpu is not None:
             phys = self.gpu_map[gpu] if self.gpu_map else gpu
             env.update(TOK8S_GPU=str(phys), LOCAL_RANK=str(phys), TOK8S_SLOT=str(gpu))

@@ -53,6 +53,7 @@ class BucketAllreduceHook:
             raise RuntimeError("BucketAllreduceHook: gradient buckets must live on the replica's "
                                "GPU; libtok8s has no CPU path")
         world = self.comm.world
+        wire_bytes = buf.numel() * (self.wire_dtype or buf.dtype).itemsize
         cur = torch.cuda.current_stream(buf.device)
         stream = self._comm_stream(buf.device) if self.overlap else cur
         if self.overlap:
@@ -76,16 +77,13 @@ class BucketAllreduceHook:
                                        elide=self.elide_identity, stream=stream)
             if self.record_events:
                 e1.record(stream)
-                wire = self.wire_dtype or buf.dtype
-                self.events.append((buf.numel() * torch.empty(0, dtype=wire).element_size(),
-                                    buf.numel() * buf.element_size(), ea, e0, e1))
+                self.events.append((wire_bytes, buf.numel() * buf.element_size(), ea, e0, e1))
             fut: torch.futures.Future = torch.futures.Future(devices=[buf.device])
             # Safe before the kernel finishes: the future records an event on the current (comm)
             # stream and consumers synchronise their streams with it (torch.futures.Future docs).
             fut.set_result(buf)
         self.buckets_seen += 1
-        wire_dt = self.wire_dtype or buf.dtype
-        self._cur_step_bytes.append(buf.numel() * torch.empty(0, dtype=wire_dt).element_size())
+        self._cur_step_bytes.append(wire_bytes)
         if bucket.is_last():
             self.last_step_bytes, self._cur_step_bytes = self._cur_step_bytes, []
         if self.buckets_seen <= 64 and self.wire_dtype in (None, buf.dtype) and \
@@ -110,10 +108,3 @@ class BucketAllreduceHook:
             out.append((wire_bytes, bucket_bytes, e0.elapsed_time(e1), ea.elapsed_time(e0)))
         self.events = []
         return out
-
-
-def register(ddp_model, comm: Communicator, **kwargs) -> BucketAllreduceHook:
-    """ddp_model.register_comm_hook(state=None, hook=BucketAllreduceHook(comm, ...))."""
-    hook = BucketAllreduceHook(comm, **kwargs)
-    ddp_model.register_comm_hook(None, hook.as_function())
-    return hook

@@ -7,72 +7,26 @@ training process keeps running; what it needs is a gradient-bucket layer that on
 communicator:
 
   * gradients live in flat buckets allocated from the replica's SYMMETRIC POOL
-    (tok_comm_symm_alloc — same allocation sequence on every replica => same offsets), parameters'
-    `.grad` are views into them (DDP's gradient_as_bucket_view layout: reverse parameter order,
-    first bucket 1 MiB then `bucket_cap_mb`, torch/nn/parallel/distributed.py:831-853);
+    (Communicator.symm_alloc — same allocation sequence on every replica => same offsets),
+    parameters' `.grad` are views into them (DDP's gradient_as_bucket_view layout: reverse parameter
+    order, first bucket 1 MiB then `bucket_cap_mb`, torch/nn/parallel/distributed.py:831-853);
   * reduce_grads() is one zero-copy tok_allreduce_bucket per bucket (scale 1/world fused);
-  * reform()/sync_params() handle elastic add/drop: survivors keep everything, a joiner builds the
+  * reform()/hand_over() handle elastic add/drop: survivors keep everything, a joiner builds the
     same bucket sequence and receives the parameters through the same kernels.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import List, Optional
 
 import torch
 
-from ._ffi import check, lib
 from .comm import Communicator
 
 
-class _RawCuda:
-    """Exposes a raw device pointer through __cuda_array_interface__ so that torch can view it."""
-
-    def __init__(self, ptr: int, nbytes: int):
-        self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1",
-                                         "data": (ptr, False), "version": 2}
-
-
 def symm_tensor(comm: Communicator, numel: int, dtype: torch.dtype) -> torch.Tensor:
-    """A flat tensor inside the replica's symmetric pool (bump-allocated, collective-consistent)."""
-    nbytes = numel * torch.empty(0, dtype=dtype).element_size()
-    ptr = C.c_void_p()
-    check(lib().tok_comm_symm_alloc(comm._h, max(nbytes, 16), C.byref(ptr)))
-    raw = torch.as_tensor(_RawCuda(ptr.value, max(nbytes, 16)), device=torch.device("cuda", comm.device))
-    return raw[:nbytes].view(dtype)
-
-
-@torch.no_grad()
-def broadcast_coalesced(comm: Communicator, tensors, root: int = 0, use_pool: bool = True) -> None:
-    """Replicate `root`'s `tensors` (one dtype, same device) into every replica's, bit for bit: packed
-    into one flat buffer, one tok_broadcast, unpacked in place on the receivers.  The flat buffer is
-    taken from the symmetric pool when it fits — the root then feeds all receivers with ONE
-    multimem.st stream through the NVSwitch — and released again (same order on every replica)."""
-    n = sum(t.numel() for t in tensors)
-    if n == 0:
-        return
-    dtype, dev = tensors[0].dtype, tensors[0].device
-    esz = tensors[0].element_size()
-    n_pad = (n * esz + 15) // 16 * 16 // esz
-    ptr = C.c_void_p()
-    pooled = use_pool and lib().tok_comm_symm_alloc(comm._h, n_pad * esz, C.byref(ptr)) == 0
-    if pooled:
-        raw = torch.as_tensor(_RawCuda(ptr.value, n_pad * esz), device=dev)
-        flat = raw.view(dtype)
-    else:
-        flat = torch.empty(n_pad, dtype=dtype, device=dev)
-    if comm.rank == root:
-        torch.cat([t.reshape(-1) for t in tensors], out=flat[:n])
-    comm.broadcast(flat, root)
-    if comm.rank != root:
-        off = 0
-        for t in tensors:
-            t.copy_(flat[off:off + t.numel()].view(t.shape))
-            off += t.numel()
-    if pooled:
-        torch.cuda.current_stream(dev).synchronize()   # the segment is recycled: nothing in flight
-        del flat, raw
-        check(lib().tok_comm_symm_free(comm._h, ptr, n_pad * esz))
+    """A flat tensor inside the replica's symmetric pool (comm.symm_alloc): the allocation every
+    gradient bucket goes through, and the name scripts and tests take pool tensors by."""
+    return comm.symm_alloc(numel, dtype)
 
 
 def bucket_assignment(sizes_bytes, keys, caps):
@@ -142,28 +96,26 @@ class ElasticDataParallel(torch.nn.Module):
     def reform(self, new_world: int, new_rank: int, member_mask: int, epoch: int) -> None:
         self.comm.reform(new_world, new_rank, member_mask, epoch)
 
-    @torch.no_grad()
-    def _broadcast_tensors(self, tensors, root: int) -> None:
-        """Coalesced broadcast (dist._broadcast_coalesced's job, torch/nn/parallel/distributed.py:1032)
-        through tok_broadcast: tensors are packed per dtype into one flat buffer, replicated
-        bit-for-bit from `root`, and unpacked in place on the receivers."""
-        me = self.comm.rank
-        by_dtype = {}
-        for t in tensors:
-            by_dtype.setdefault(t.dtype, []).append(t)
-        for dtype, ts in by_dtype.items():
-            n = sum(t.numel() for t in ts)
-            if n == 0:
-                continue
-            broadcast_coalesced(self.comm, ts, root, use_pool=self.pool_broadcast)
+    def hand_over(self, optimizer: torch.optim.Optimizer, step: int, root: int = 0) -> int:
+        """What every member runs right after a re-form or a join, before its next step: `root`'s
+        parameters, buffers, optimizer state and step counter to the whole group, in this order on
+        every replica, then a device synchronize.  Returns `root`'s step."""
+        self.sync_params(root)
+        self.sync_optimizer_state(optimizer, root)
+        cell = torch.zeros(2, dtype=torch.int64, device=next(self.module.parameters()).device)
+        cell[0] = step
+        self.comm.broadcast(cell, root)
+        torch.cuda.synchronize()
+        return int(cell[0].item())
 
     @torch.no_grad()
     def sync_params(self, root: int = 0) -> None:
         """Replicate rank `root`'s parameters and ALL buffers (BatchNorm's integer
         num_batches_tracked included) to the whole group — what a replica that joins at an elastic
         re-form needs before its first step."""
-        self._broadcast_tensors([p.data for p in self.module.parameters()] +
-                                [b for b in self.module.buffers()], root)
+        self.comm.broadcast_coalesced([p.data for p in self.module.parameters()] +
+                                      [b for b in self.module.buffers()], root,
+                                      use_pool=self.pool_broadcast)
 
     @torch.no_grad()
     def sync_optimizer_state(self, optimizer: torch.optim.Optimizer, root: int = 0) -> None:
@@ -209,7 +161,7 @@ class ElasticDataParallel(torch.nn.Module):
                         tensors.append(st[name])
                 else:                    # python number
                     scalars.append((st, name, v))
-        self._broadcast_tensors(tensors, root)
+        self.comm.broadcast_coalesced(tensors, root, use_pool=self.pool_broadcast)
         if scalars:
             flat = torch.tensor([float(v) for _, _, v in scalars], dtype=torch.float64, device=dev)
             self.comm.broadcast(flat, root)

@@ -8,6 +8,7 @@ the single-box controller assigns (one replica per GPU).
 """
 from __future__ import annotations
 
+import contextlib
 import os
 from dataclasses import dataclass
 from typing import Optional
@@ -15,6 +16,8 @@ from typing import Optional
 import torch
 import torch.distributed as dist
 
+from . import membership
+from .membership import membership_update, wait_for_membership
 from .comm import Communicator, default_rendezvous_path
 from .ddp_hook import BucketAllreduceHook
 
@@ -33,38 +36,33 @@ class Replica:
              **ddp_kwargs):
         """DistributedDataParallel(model) whose gradient buckets go through libtok8s.
 
-        zero_copy: allocate DDP's bucket storage inside this replica's symmetric pool (a
-        torch.cuda.MemPool over libtok8s' pluggable allocator), so that with
+        zero_copy (world > 1, no wire_dtype): allocate DDP's bucket storage inside this replica's
+        symmetric pool (a torch.cuda.MemPool over libtok8s' pluggable allocator), so that with
         gradient_as_bucket_view the gradients are produced directly in peer-mapped memory and the
-        exchange needs no staging pass.  Buckets that end up outside the pool (or a pool that cannot
-        be created) silently take the staged path — results are identical."""
+        exchange needs no staging pass.  A bucket that ends up outside the pool takes the staged
+        path, with identical results.  A pool that cannot be created raises rather than change
+        kernels silently: pass zero_copy=False to ask for the staged path."""
         from torch.nn.parallel import DistributedDataParallel as DDP
-        scope = None
-        if zero_copy and self.world > 1 and wire_dtype is None:
-            # a MemPool that cannot be created is an error, not a reason to change kernels silently:
-            # pass zero_copy=False to ask for the staged path
+        pooled = zero_copy and self.world > 1 and wire_dtype is None
+        if pooled:
             self.comm.mem_pool()
-            scope = self.comm.symmetric
         # DDP's own start-up broadcast (dist._broadcast_coalesced over the process group) is replaced
         # by tok_broadcast: init_sync=False skips it, broadcast_module_states() does it over NVLink
         ddp_kwargs.setdefault("init_sync", False)
         if self.world > 1 and not ddp_kwargs["init_sync"]:
             self.broadcast_module_states(model)
-        if scope is None:
+        scope = self.comm.symmetric if pooled else contextlib.nullcontext
+        with scope():
             ddp = DDP(model, device_ids=[self.device.index], bucket_cap_mb=bucket_cap_mb,
                       gradient_as_bucket_view=True, **ddp_kwargs)
-        else:
-            with scope():
-                ddp = DDP(model, device_ids=[self.device.index], bucket_cap_mb=bucket_cap_mb,
-                          gradient_as_bucket_view=True, **ddp_kwargs)
-            # DDP re-allocates its buckets once, after the first iteration, from
-            # DistributedDataParallel._pre_forward -> reducer._rebuild_buckets(): keep that in the pool
-            inner = getattr(ddp, "_pre_forward", None)
-            if inner is not None:
-                def _pre_forward(*a, **k):
-                    with scope():
-                        return inner(*a, **k)
-                ddp._pre_forward = _pre_forward
+        # DDP re-allocates its buckets once, after the first iteration, from
+        # DistributedDataParallel._pre_forward -> reducer._rebuild_buckets(): keep that in the pool
+        inner = getattr(ddp, "_pre_forward", None)
+        if pooled and inner is not None:
+            def _pre_forward(*a, **k):
+                with scope():
+                    return inner(*a, **k)
+            ddp._pre_forward = _pre_forward
         hook = BucketAllreduceHook(self.comm, wire_dtype=wire_dtype, overlap=overlap,
                                    record_events=record_events, elide_identity=elide_identity)
         ddp.register_comm_hook(None, hook.as_function())
@@ -73,33 +71,8 @@ class Replica:
     def broadcast_module_states(self, module: torch.nn.Module, root: int = 0) -> None:
         """Rank `root`'s parameters and buffers to every replica (DDP's _sync_module_states,
         torch/nn/parallel/distributed.py:1032, over tok_broadcast instead of the process group)."""
-        from .elastic_dp import broadcast_coalesced
-        by_dtype = {}
-        for t in list(module.parameters()) + list(module.buffers()):
-            by_dtype.setdefault(t.dtype, []).append(t.data)
-        for ts in by_dtype.values():
-            broadcast_coalesced(self.comm, ts, root)
-
-    def poll_membership(self):
-        """Elastic add/drop without a restart, single-replica view: read the membership epoch file
-        the controller writes next to the rendezvous socket (controller.Controller._publish_membership)
-        and, when the epoch moved, re-form the peer group in place (tok_comm_reform).  Returns the new
-        (rank, world), or None when nothing changed or this replica is no longer a member.
-        Replicas that are in the middle of a training loop must agree on the STEP at which they
-        re-form — use poll_membership_collective()."""
-        import json
-        try:
-            with open(self.comm.rendezvous_path + ".members") as f:
-                doc = json.load(f)
-        except (OSError, ValueError):
-            return None
-        step = membership_update(doc, os.environ.get("TOK8S_REPLICA", ""), self.comm.caps().epoch)
-        if step is None:
-            return None
-        new_world, new_rank, mask, epoch = step
-        self.comm.reform(new_world, new_rank, mask, epoch)
-        self.rank, self.world = new_rank, new_world
-        return self.rank, self.world
+        self.comm.broadcast_coalesced([t.data for t in list(module.parameters()) +
+                                       list(module.buffers())], root)
 
     def poll_membership_collective(self):
         """The same decision taken by the whole group at one step boundary: rank 0's view of the
@@ -108,15 +81,11 @@ class Replica:
         would wait in the rendezvous while they wait for it in the gradient exchange.
         Returns ("reformed", rank, world), ("dropped",) when the new membership no longer lists this
         replica (it must stop using the communicator and exit), or None."""
-        import json
         import time
+        rdzv = self.comm.rendezvous_path
         cur = self.comm.caps().epoch
-        seen = 0
-        try:
-            with open(self.comm.rendezvous_path + ".members") as f:
-                seen = int(json.load(f).get("epoch", 0))
-        except (OSError, ValueError):
-            seen = 0
+        doc = membership.read(rdzv)
+        seen = 0 if doc is None else int(doc.get("epoch", 0))
         if self.world > 1:
             if getattr(self, "_epoch_cell", None) is None:
                 self._epoch_cell = torch.zeros(2, dtype=torch.int64, device=self.device)
@@ -128,13 +97,9 @@ class Replica:
         me = os.environ.get("TOK8S_REPLICA", "")
         deadline = time.time() + 30.0
         while True:                                      # rank 0 saw it: the file is there
-            try:
-                with open(self.comm.rendezvous_path + ".members") as f:
-                    doc = json.load(f)
-                if int(doc.get("epoch", 0)) >= seen:
-                    break
-            except (OSError, ValueError):
-                pass
+            doc = membership.read(rdzv)
+            if doc is not None and int(doc.get("epoch", 0)) >= seen:
+                break
             if time.time() > deadline:
                 raise TimeoutError("membership epoch %d announced by rank 0 is not readable" % seen)
             time.sleep(0.005)
@@ -160,15 +125,6 @@ def report_metric(**record) -> None:
     torch_on_k8s_allreduce_busbw_gbps / torch_on_k8s_reform_latency_seconds."""
     import json
     print("TOK8S_METRIC " + json.dumps(record), flush=True)
-
-
-def membership_update(doc: dict, replica_name: str, current_epoch: int):
-    """Pure decision behind Replica.poll_membership: (new_world, new_rank, member_mask, epoch) for
-    tok_comm_reform, or None when the published epoch is not newer / this replica was dropped."""
-    if int(doc.get("epoch", 0)) <= current_epoch or replica_name not in doc.get("ranks", {}):
-        return None
-    return int(doc["world"]), int(doc["ranks"][replica_name]), int(doc.get("survivor_mask", 0)), \
-        int(doc["epoch"])
 
 
 def init_replica(job_id: Optional[str] = None, *, device: Optional[int] = None,
@@ -204,31 +160,8 @@ def init_replica(job_id: Optional[str] = None, *, device: Optional[int] = None,
         # (a scale-out that was reverted first never lists this replica)
         torch.zeros(1, device=dev)
         replica = os.environ.get("TOK8S_REPLICA", "")
-        with open("%s.ready.%s" % (rdzv, replica), "w") as f:
-            f.write(str(epoch))
+        membership.mark_ready(rdzv, replica, epoch)
         rank, world, epoch = wait_for_membership(rdzv, replica, epoch)
     comm = Communicator(job_id, rank, world, device, max_world=max_world, rendezvous_path=rdzv,
                         epoch=epoch)
     return Replica(rank=rank, world=world, device=dev, comm=comm, job_id=job_id)
-
-
-def wait_for_membership(rdzv_path: str, replica_name: str, min_epoch: int,
-                        timeout_s: Optional[float] = None):
-    """(rank, world, epoch) of the first published membership with epoch >= min_epoch that lists
-    `replica_name` (controller.Controller._publish_membership writes <rendezvous>.members)."""
-    import json
-    import time
-    deadline = time.time() + (timeout_s if timeout_s is not None else
-                              float(os.environ.get("TOK_RDZV_TIMEOUT_S", "120")))
-    while True:
-        try:
-            with open(rdzv_path + ".members") as f:
-                doc = json.load(f)
-            if int(doc.get("epoch", 0)) >= min_epoch and replica_name in doc.get("ranks", {}):
-                return int(doc["ranks"][replica_name]), int(doc["world"]), int(doc["epoch"])
-        except (OSError, ValueError):
-            pass
-        if time.time() > deadline:
-            raise TimeoutError("no membership listing %s at epoch >= %d was published under %s" %
-                               (replica_name, min_epoch, rdzv_path + ".members"))
-        time.sleep(0.02)

@@ -78,21 +78,15 @@ def main() -> int:
     edp = ElasticDataParallel(model, rep.comm, bucket_cap_mb=25)
     opt = torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
     sampler = ReplicaSampler(a.steps * a.batch * 8, rep.world, rep.rank, seed=0)
-    cell = torch.zeros(2, dtype=torch.int64, device=dev)   # [next step] handed to joiners by rank 0
 
     def log(**kw):
         print("TOK8S_STEP " + json.dumps(dict(replica=name, rank=rep.rank, world=rep.world,
                                               t=time.time(), **kw)), flush=True)
 
     def hand_over(step):
-        """after a re-form / join: rank 0's model, optimizer state and step counter to everybody"""
+        """edp.hand_over after a re-form / join, timed: (rank 0's step, seconds)"""
         t0 = time.time()
-        edp.sync_params(0)
-        edp.sync_optimizer_state(opt, 0)
-        cell[0] = step
-        rep.comm.broadcast(cell, 0)
-        torch.cuda.synchronize()
-        return int(cell[0].item()), time.time() - t0
+        return edp.hand_over(opt, step), time.time() - t0
 
     step = 0
     fresh = False
