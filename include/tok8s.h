@@ -182,6 +182,29 @@ int tok_comm_use_as_pool(tok_comm_t* comm);
 void* tok_pool_malloc(ptrdiff_t size, int device, void* cuda_stream);
 void tok_pool_free(void* ptr, size_t size, int device, void* cuda_stream);
 
+/* Batch-norm forward (training) fused with ReLU and the residual add, for NHWC bf16 activations seen
+ * as [rows = N*H*W, channels] (torch_on_k8s_b200/fused_bn.py).  `mean` and `var` are the float
+ * batch statistics ATen's channels_last statistics kernel produced (biased variance); every call
+ * writes invstd = rsqrt(var + eps) to `invstd` (float[channels]) and
+ *   tok_bn_relu_fwd:      y = relu(bn(x))
+ *   tok_bn_add_relu_fwd:  y = relu(bn(x) + residual)
+ *   tok_bn2_add_relu_fwd: y = relu(bn(x) + bn_d(xd))
+ * rounding every intermediate to bf16 where the unfused PyTorch ops do, so that y is bit-identical
+ * to theirs.  weight and bias are bf16[channels].  Activations and y must be 16-byte aligned and
+ * channels a multiple of 8 (TOK_ERR_ALIGN).  Enqueued on `cuda_stream`, no synchronisation;
+ * TOK_ERR_NO_DEVICE without a GPU. */
+int tok_bn_relu_fwd(const void* x, const float* mean, const float* var, const void* weight,
+                    const void* bias, float eps, float* invstd, void* y, int64_t rows,
+                    int channels, void* cuda_stream);
+int tok_bn_add_relu_fwd(const void* x, const float* mean, const float* var, const void* weight,
+                        const void* bias, float eps, float* invstd, const void* residual, void* y,
+                        int64_t rows, int channels, void* cuda_stream);
+int tok_bn2_add_relu_fwd(const void* x, const float* mean, const float* var, const void* weight,
+                         const void* bias, float eps, float* invstd, const void* xd,
+                         const float* mean_d, const float* var_d, const void* weight_d,
+                         const void* bias_d, float eps_d, float* invstd_d, void* y, int64_t rows,
+                         int channels, void* cuda_stream);
+
 /* Which algorithm AUTO picks for `wire_bytes` on this communicator. */
 int tok_allreduce_algo(tok_comm_t* comm, size_t wire_bytes, int* algo);
 /* Number of kernels this communicator has launched so far (bench.py's gpu_launches): exchange,

@@ -107,6 +107,11 @@ PROTOTYPES = {
     "tok_broadcast": (C.c_int, [_P, _P, C.c_size_t, C.c_int, _P]),
     "tok_comm_stats": (C.c_int, [_P, C.POINTER(Stats)]),
     "tok_comm_symm_free": (C.c_int, [_P, _P, C.c_size_t]),
+    "tok_bn_relu_fwd": (C.c_int, [_P, _P, _P, _P, _P, C.c_float, _P, _P, C.c_int64, C.c_int, _P]),
+    "tok_bn_add_relu_fwd": (C.c_int, [_P, _P, _P, _P, _P, C.c_float, _P, _P, _P, C.c_int64,
+                                      C.c_int, _P]),
+    "tok_bn2_add_relu_fwd": (C.c_int, [_P, _P, _P, _P, _P, C.c_float, _P, _P, _P, _P, _P, _P,
+                                       C.c_float, _P, _P, C.c_int64, C.c_int, _P]),
     "tok_allreduce_algo": (C.c_int, [_P, C.c_size_t, _IP]),
     "tok_comm_launches": (C.c_int, [_P, C.POINTER(C.c_uint64)]),
     "tok_comm_symm_alloc": (C.c_int, [_P, C.c_size_t, _PP]),

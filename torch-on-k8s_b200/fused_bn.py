@@ -1,0 +1,152 @@
+"""Batch norm fused with ReLU and the residual add, for ResNet-style training in NHWC bf16.
+
+    bn_relu(x, bn)                 == relu_(bn(x))
+    bn_add_relu(x, bn, r)          == relu_(bn(x) + r)
+    bn2_add_relu(x, bn, xd, bnd)   == relu_(bn(x) + bnd(xd))
+
+`bn` / `bnd` are ordinary nn.BatchNorm2d modules and are used as they are: their parameters get the
+gradients, their running statistics and `num_batches_tracked` are updated exactly as the module's own
+forward would update them.  The results, the gradients and the updated buffers are bit-identical to
+the unfused composition, so swapping these in changes no number of a training run.
+
+What is fused: the forward elementwise passes.  The batch statistics still come from ATen's
+channels_last statistics kernel (`torch.batch_norm_update_stats`, which also updates the running
+statistics); one libtok8s kernel then applies the normalisation with ATen's exact float expression,
+adds the residual (or the second, downsample batch norm) and applies the ReLU, writing one bf16
+tensor where the stock composition writes and re-reads two or three.  The backward is the stock
+one: `threshold_backward` on the saved output, then `native_batch_norm_backward` with the saved
+mean and invstd, saving the same activations stock autograd saves (the batch-norm inputs and the
+ReLU output).
+
+The fused path is taken when the inputs allow it: CUDA, bf16 activations and batch-norm tensors,
+channels_last-contiguous 4-D activations with C % 8 == 0 and 16-byte aligned data, a module in
+training mode that tracks running statistics with a fixed momentum.  Anything else (CPU, eval, fp32,
+NCHW, ...) runs the stock composition.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import torch
+import torch.nn.functional as F
+from torch.autograd.function import once_differentiable
+
+from . import _ffi
+
+_INT32_MAX = (1 << 31) - 1
+
+
+def _fusable_bn(bn: torch.nn.Module, x: torch.Tensor) -> bool:
+    if not (bn.training and bn.track_running_stats and bn.affine and bn.momentum is not None
+            and bn.running_mean is not None and bn.num_batches_tracked is not None):
+        return False
+    for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var):
+        if t.dtype != torch.bfloat16 or t.device != x.device or not t.is_contiguous():
+            return False
+    return True
+
+
+def _fusable_act(x: torch.Tensor) -> bool:
+    return (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.shape[1] % 8 == 0
+            and x.stride(1) == 1 and x.is_contiguous(memory_format=torch.channels_last)
+            and 1 < x.numel() // x.shape[1] and x.numel() <= _INT32_MAX
+            and x.data_ptr() % 16 == 0)
+
+
+def _same(a: torch.Tensor, b: torch.Tensor) -> bool:
+    return (_fusable_act(b) and a.shape == b.shape and a.device == b.device)
+
+
+def _stats(x: torch.Tensor, bn: torch.nn.Module):
+    """Batch mean and biased variance (float) from ATen's channels_last statistics kernel, with the
+    running statistics and num_batches_tracked updated as nn.BatchNorm2d.forward updates them."""
+    bn.num_batches_tracked.add_(1)
+    return torch.batch_norm_update_stats(x, bn.running_mean, bn.running_var, bn.momentum)
+
+
+def _ptr(t):
+    return C.c_void_p(t.data_ptr())
+
+
+def _bn_backward(g, x, bn, mean, invstd, mask):
+    return torch.ops.aten.native_batch_norm_backward(
+        g, x, bn.weight, bn.running_mean, bn.running_var, mean, invstd, True, bn.eps, mask)
+
+
+class _BnAddRelu(torch.autograd.Function):
+    """y = relu(bn(x) [+ r | + bnd(xd)]); the residual is `r` (mode 1) or `xd` through `bnd` (mode 2)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, other, weight_d, bias_d, bn, bnd, mode):
+        rows, ch = x.numel() // x.shape[1], x.shape[1]
+        mean, var = _stats(x, bn)
+        invstd = torch.empty_like(mean)
+        y = torch.empty_like(x)
+        lib = _ffi.lib()
+        with torch.cuda.device(x.device):
+            stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
+            if mode == 0:
+                rc = lib.tok_bn_relu_fwd(_ptr(x), _ptr(mean), _ptr(var), _ptr(weight), _ptr(bias),
+                                         bn.eps, _ptr(invstd), _ptr(y), rows, ch, stream)
+            elif mode == 1:
+                rc = lib.tok_bn_add_relu_fwd(_ptr(x), _ptr(mean), _ptr(var), _ptr(weight),
+                                             _ptr(bias), bn.eps, _ptr(invstd), _ptr(other), _ptr(y),
+                                             rows, ch, stream)
+            else:
+                mean_d, var_d = _stats(other, bnd)
+                invstd_d = torch.empty_like(mean_d)
+                rc = lib.tok_bn2_add_relu_fwd(_ptr(x), _ptr(mean), _ptr(var), _ptr(weight),
+                                              _ptr(bias), bn.eps, _ptr(invstd), _ptr(other),
+                                              _ptr(mean_d), _ptr(var_d), _ptr(weight_d),
+                                              _ptr(bias_d), bnd.eps, _ptr(invstd_d), _ptr(y), rows,
+                                              ch, stream)
+        _ffi.check(rc)
+        ctx.bn, ctx.bnd, ctx.mode = bn, bnd, mode
+        if mode == 2:
+            ctx.save_for_backward(x, mean, invstd, other, mean_d, invstd_d, y)
+        else:
+            ctx.save_for_backward(x, mean, invstd, y)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        need = ctx.needs_input_grad
+        saved = ctx.saved_tensors
+        y = saved[-1]
+        g = torch.ops.aten.threshold_backward(gy, y, 0)
+        dxd = dwd = dbd = dr = None
+        if ctx.mode == 2:
+            x, mean, invstd, xd, mean_d, invstd_d, _ = saved
+            # the downsample branch first, as the unfused graph orders it
+            dxd, dwd, dbd = _bn_backward(g, xd, ctx.bnd, mean_d, invstd_d, [need[3], need[4], need[5]])
+        else:
+            x, mean, invstd, _ = saved
+            if ctx.mode == 1 and need[3]:
+                dr = g
+        dx, dw, db = _bn_backward(g, x, ctx.bn, mean, invstd, [need[0], need[1], need[2]])
+        if ctx.mode == 2:
+            return dx, dw, db, dxd, dwd, dbd, None, None, None
+        return dx, dw, db, dr, None, None, None, None, None
+
+
+def bn_relu(x: torch.Tensor, bn: torch.nn.Module) -> torch.Tensor:
+    """relu(bn(x)), fused on CUDA bf16 channels_last training inputs."""
+    if _fusable_act(x) and _fusable_bn(bn, x):
+        return _BnAddRelu.apply(x, bn.weight, bn.bias, None, None, None, bn, None, 0)
+    return F.relu(bn(x), inplace=True)
+
+
+def bn_add_relu(x: torch.Tensor, bn: torch.nn.Module, r: torch.Tensor) -> torch.Tensor:
+    """relu(bn(x) + r), fused on CUDA bf16 channels_last training inputs."""
+    if _fusable_act(x) and _fusable_bn(bn, x) and _same(x, r):
+        return _BnAddRelu.apply(x, bn.weight, bn.bias, r, None, None, bn, None, 1)
+    return F.relu(bn(x) + r, inplace=True)
+
+
+def bn2_add_relu(x: torch.Tensor, bn: torch.nn.Module, xd: torch.Tensor,
+                 bnd: torch.nn.Module) -> torch.Tensor:
+    """relu(bn(x) + bnd(xd)), fused on CUDA bf16 channels_last training inputs."""
+    if _fusable_act(x) and _fusable_bn(bn, x) and _same(x, xd) and _fusable_bn(bnd, xd):
+        return _BnAddRelu.apply(x, bn.weight, bn.bias, xd, bnd.weight, bnd.bias, bn, bnd, 2)
+    return F.relu(bn(x) + bnd(xd), inplace=True)

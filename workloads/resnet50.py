@@ -1,10 +1,16 @@
 """ResNet-50 (He et al. 2015, v1.5 stride placement as in torchvision) in plain torch.nn — the model
 BASELINE.json config 2 names.  25,557,032 parameters, 161 parameter tensors; random init (no
-network for checkpoints)."""
+network for checkpoints).
+
+Every batch norm is applied through torch_on_k8s_b200.fused_bn together with the ReLU and residual
+add that follow it: on CUDA bf16 channels_last training inputs that is one fused libtok8s kernel
+per site, bit-identical to the unfused ops; anything else runs the plain nn composition."""
 from __future__ import annotations
 
 import torch
 import torch.nn as nn
+
+from torch_on_k8s_b200.fused_bn import bn2_add_relu, bn_add_relu, bn_relu
 
 
 class Bottleneck(nn.Module):
@@ -22,13 +28,14 @@ class Bottleneck(nn.Module):
         self.downsample = downsample
 
     def forward(self, x):
-        identity = x
-        out = self.relu(self.bn1(self.conv1(x)))
-        out = self.relu(self.bn2(self.conv2(out)))
-        out = self.bn3(self.conv3(out))
+        out = bn_relu(self.conv1(x), self.bn1)
+        out = bn_relu(self.conv2(out), self.bn2)
+        out = self.conv3(out)
         if self.downsample is not None:
-            identity = self.downsample(x)
-        return self.relu(out + identity)
+            # downsample = Sequential(conv, bn): its batch norm is fused into the residual add
+            conv_d, bn_d = self.downsample
+            return bn2_add_relu(out, self.bn3, conv_d(x), bn_d)
+        return bn_add_relu(out, self.bn3, x)
 
 
 class ResNet50(nn.Module):
@@ -65,7 +72,7 @@ class ResNet50(nn.Module):
         return nn.Sequential(*layers)
 
     def forward(self, x):
-        x = self.maxpool(self.relu(self.bn1(self.conv1(x))))
+        x = self.maxpool(bn_relu(self.conv1(x), self.bn1))
         x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
         x = torch.flatten(self.avgpool(x), 1)
         return self.fc(x)
