@@ -205,6 +205,33 @@ int tok_bn2_add_relu_fwd(const void* x, const float* mean, const float* var, con
                          const void* bias_d, float eps_d, float* invstd_d, void* y, int64_t rows,
                          int channels, void* cuda_stream);
 
+/* SGD step on fp32 master weights for bf16 / f16 parameters (torch_on_k8s_b200/optim.py), one launch
+ * per gradient bucket.  For every element of every segment it produces the bits of
+ *   torch.optim.SGD(masters, lr, momentum, dampening, weight_decay, nesterov).step()   (foreach)
+ *   param.copy_(master)                                                                 (RNE)
+ * with grad = f32(segment.grad) as the master's gradient.  `fresh` != 0 means the momentum buffers
+ * hold nothing yet: they are set to the (weight-decayed) gradient, as torch's first step clones it.
+ * The hyperparameters are torch's Python floats; they are rounded to float as ATen rounds them.
+ * `segments` is a DEVICE array of `count` entries; entry k's `chunk0` must be the sum of
+ * ceil(numel / TOK_SGD_CHUNK) over the entries before it and `chunks` that sum over all entries
+ * (one CTA per chunk).  Segments may start at any element; 16-byte vector loads are used where the
+ * pointers allow.  Returns TOK_ERR_INVALID for bad hyperparameters (negative or non-finite lr,
+ * momentum or weight_decay; nesterov without momentum or with dampening), a dtype other than
+ * TOK_BF16 / TOK_F16 or an empty table, TOK_ERR_NO_DEVICE without a GPU.  Enqueued on
+ * `cuda_stream`, no synchronisation. */
+#define TOK_SGD_CHUNK 4096
+typedef struct tok_sgd_segment {
+  const void* grad; /* bf16 / f16[numel], the parameter's gradient (anywhere in its bucket)       */
+  void* param;      /* bf16 / f16[numel], written                                                 */
+  float* master;    /* fp32[numel], read and written                                              */
+  float* momentum;  /* fp32[numel], read (unless fresh) and written; unused when momentum == 0    */
+  int64_t numel;
+  int64_t chunk0;   /* index of this segment's first chunk                                        */
+} tok_sgd_segment_t;
+int tok_sgd_master_step(const tok_sgd_segment_t* segments, int count, int64_t chunks, int dtype,
+                        double lr, double momentum, double dampening, double weight_decay,
+                        int nesterov, int fresh, void* cuda_stream);
+
 /* Which algorithm AUTO picks for `wire_bytes` on this communicator. */
 int tok_allreduce_algo(tok_comm_t* comm, size_t wire_bytes, int* algo);
 /* Number of kernels this communicator has launched so far (bench.py's gpu_launches): exchange,

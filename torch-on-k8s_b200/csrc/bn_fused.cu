@@ -149,6 +149,8 @@ __global__ void __launch_bounds__(kBnThreads) bn_fused_fwd_kernel(const BnArgs p
   }
 }
 
+}  // namespace
+
 // ---- host side --------------------------------------------------------------------------------
 int device_ready() {
   static const int ok = [] {
@@ -157,6 +159,8 @@ int device_ready() {
   }();
   return ok;
 }
+
+namespace {
 
 struct DevInfo {
   std::atomic<int> sms{0};

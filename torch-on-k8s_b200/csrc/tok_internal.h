@@ -88,6 +88,9 @@ int launch_barrier_bench(int ctas, const KArgs& args, void* stream);  // profili
 // Shared memory the TMA-staged local kernel asks for (opt-in dynamic shared memory).
 size_t local_tma_smem_bytes();
 
+// 1 when the process sees a CUDA device (bn_fused.cu); the kernels' entry points check it last
+int device_ready();
+
 // error plumbing (comm.cpp)
 void set_error(const char* fmt, ...);
 int fail(int code, const char* fmt, ...);

@@ -23,12 +23,17 @@ class BucketAllreduceHook:
     overlap=True launches on a dedicated communication stream so that the exchange of bucket k
     overlaps the backward kernels that are still producing bucket k+1 (DDP's own overlap model);
     the returned CUDA-aware Future carries the event consumers must wait on.
+
+    optimizer (a MasterWeightSGD): each bucket's optimizer step is enqueued on the same stream right
+    behind its exchange, before the Future is set; optimizer.step() then only orders the current
+    stream after that stream.
     """
 
     def __init__(self, comm: Communicator, *, wire_dtype: Optional[torch.dtype] = None,
                  overlap: bool = True, record_events: bool = False, algo: int = 0,
-                 elide_identity: bool = True):
+                 elide_identity: bool = True, optimizer=None):
         self.comm = comm
+        self.optimizer = optimizer
         self.wire_dtype = wire_dtype
         self.overlap = overlap
         self.algo = algo
@@ -78,6 +83,13 @@ class BucketAllreduceHook:
             if self.record_events:
                 e1.record(stream)
                 self.events.append((wire_bytes, buf.numel() * buf.element_size(), ea, e0, e1))
+            if self.optimizer is not None:
+                # GradBucket.gradients() are contiguous views; with gradient_as_bucket_view the
+                # gradient is laid out in the bucket as its parameter is in memory (channels_last too)
+                params = bucket.parameters()
+                grads = [g.as_strided(p.shape, p.stride())
+                         for p, g in zip(params, bucket.gradients())]
+                self.optimizer.step_bucket(params, grads, bucket.index(), stream)
             fut: torch.futures.Future = torch.futures.Future(devices=[buf.device])
             # Safe before the kernel finishes: the future records an event on the current (comm)
             # stream and consumers synchronise their streams with it (torch.futures.Future docs).

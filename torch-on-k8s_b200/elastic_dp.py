@@ -62,6 +62,7 @@ class ElasticDataParallel(torch.nn.Module):
         self.algo = algo
         self.pool_broadcast = pool_broadcast   # state hand-over through pool buffers (zero-copy path)
         self.buckets: List[torch.Tensor] = []
+        self.bucket_params: List[List[torch.nn.Parameter]] = []   # the parameters of each bucket
         self._assign(bucket_cap_mb << 20, first_bucket_mb << 20)
 
     def _assign(self, cap: int, first_cap: int) -> None:
@@ -78,6 +79,7 @@ class ElasticDataParallel(torch.nn.Module):
                 p.grad = flat[off:off + p.numel()].view(p.shape)
                 off += (p.numel() + 7) // 8 * 8
             self.buckets.append(flat)
+            self.bucket_params.append(ps)
 
     def forward(self, *args, **kwargs):
         return self.module(*args, **kwargs)
@@ -86,11 +88,16 @@ class ElasticDataParallel(torch.nn.Module):
         for b in self.buckets:
             b.zero_()
 
-    def reduce_grads(self, stream: Optional[torch.cuda.Stream] = None) -> None:
-        """Average the gradient buckets across the current peer group (in place, zero-copy)."""
+    def reduce_grads(self, stream: Optional[torch.cuda.Stream] = None, optimizer=None) -> None:
+        """Average the gradient buckets across the current peer group (in place, zero-copy).
+        optimizer (a MasterWeightSGD): each bucket's step is enqueued right behind its exchange;
+        optimizer.step() then launches nothing for these parameters."""
         world = self.comm.world
-        for b in self.buckets:   # PRE scale: the same function as built-in DDP at every world size
+        for k, b in enumerate(self.buckets):   # PRE scale: the same function as built-in DDP
             self.comm.allreduce_bucket(b, b, scale=1.0 / world, algo=self.algo, stream=stream)
+            if optimizer is not None:
+                ps = self.bucket_params[k]
+                optimizer.step_bucket(ps, [p.grad for p in ps], k, stream)
 
     # ---- elastic ------------------------------------------------------------------------------
     def reform(self, new_world: int, new_rank: int, member_mask: int, epoch: int) -> None:
@@ -130,7 +137,7 @@ class ElasticDataParallel(torch.nn.Module):
         # layout = for every parameter, which tensor-valued state keys the root holds (bitmask over
         # the sorted union of known keys; python scalars such as `step` ints travel as f64)
         keys = ["momentum_buffer", "exp_avg", "exp_avg_sq", "max_exp_avg_sq", "step", "square_avg",
-                "acc_delta", "sum"]
+                "acc_delta", "sum", "master_param"]
         layout = torch.zeros(len(params), dtype=torch.int64, device=dev)
         if me == root:
             for i, p in enumerate(params):
@@ -156,8 +163,9 @@ class ElasticDataParallel(torch.nn.Module):
                     if name == "step":
                         st[name] = torch.zeros((), dtype=torch.float32)
                         scalars.append((st, name, st[name]))
-                    else:
-                        st[name] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    else:   # a master-weight optimizer keeps its state in the master's dtype
+                        st[name] = torch.zeros_like(st.get("master_param", p),
+                                                    memory_format=torch.preserve_format)
                         tensors.append(st[name])
                 else:                    # python number
                     scalars.append((st, name, v))

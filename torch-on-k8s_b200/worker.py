@@ -33,7 +33,7 @@ class Replica:
     def wrap(self, model: torch.nn.Module, *, bucket_cap_mb: int = 25,
              wire_dtype: Optional[torch.dtype] = None, overlap: bool = True,
              record_events: bool = False, zero_copy: bool = True, elide_identity: bool = True,
-             **ddp_kwargs):
+             optimizer=None, **ddp_kwargs):
         """DistributedDataParallel(model) whose gradient buckets go through libtok8s.
 
         zero_copy (world > 1, no wire_dtype): allocate DDP's bucket storage inside this replica's
@@ -41,7 +41,11 @@ class Replica:
         gradient_as_bucket_view the gradients are produced directly in peer-mapped memory and the
         exchange needs no staging pass.  A bucket that ends up outside the pool takes the staged
         path, with identical results.  A pool that cannot be created raises rather than change
-        kernels silently: pass zero_copy=False to ask for the staged path."""
+        kernels silently: pass zero_copy=False to ask for the staged path.
+
+        optimizer (a torch_on_k8s_b200.optim.MasterWeightSGD over the model's parameters): the hook
+        steps each bucket's parameters right behind the bucket's exchange; optimizer.step() then
+        launches nothing for them."""
         from torch.nn.parallel import DistributedDataParallel as DDP
         pooled = zero_copy and self.world > 1 and wire_dtype is None
         if pooled:
@@ -51,6 +55,9 @@ class Replica:
         ddp_kwargs.setdefault("init_sync", False)
         if self.world > 1 and not ddp_kwargs["init_sync"]:
             self.broadcast_module_states(model)
+        if self.world > 1 and optimizer is not None:   # the masters follow rank 0's parameters
+            self.comm.broadcast_coalesced([optimizer.state[p]["master_param"]
+                                           for g in optimizer.param_groups for p in g["params"]], 0)
         scope = self.comm.symmetric if pooled else contextlib.nullcontext
         with scope():
             ddp = DDP(model, device_ids=[self.device.index], bucket_cap_mb=bucket_cap_mb,
@@ -64,7 +71,8 @@ class Replica:
                     return inner(*a, **k)
             ddp._pre_forward = _pre_forward
         hook = BucketAllreduceHook(self.comm, wire_dtype=wire_dtype, overlap=overlap,
-                                   record_events=record_events, elide_identity=elide_identity)
+                                   record_events=record_events, elide_identity=elide_identity,
+                                   optimizer=optimizer)
         ddp.register_comm_hook(None, hook.as_function())
         return ddp, hook
 

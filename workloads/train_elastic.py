@@ -57,6 +57,9 @@ def main() -> int:
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--lr", type=float, default=1e-3)
     ap.add_argument("--log-every", type=int, default=5)
+    ap.add_argument("--master-weights", action="store_true",
+                    help="bf16 models: SGD on fp32 master weights, stepped behind each bucket's "
+                         "exchange (torch_on_k8s_b200.optim.MasterWeightSGD)")
     a = ap.parse_args()
 
     t_proc = time.time()
@@ -76,7 +79,11 @@ def main() -> int:
     joined_at_epoch = rep.comm.caps().epoch
     name = os.environ.get("TOK8S_REPLICA", "replica-%d" % rep.rank)
     edp = ElasticDataParallel(model, rep.comm, bucket_cap_mb=25)
-    opt = torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
+    if a.master_weights:
+        from torch_on_k8s_b200.optim import MasterWeightSGD
+        opt = MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9)
+    else:
+        opt = torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
     sampler = ReplicaSampler(a.steps * a.batch * 8, rep.world, rep.rank, seed=0)
 
     def log(**kw):
@@ -116,7 +123,7 @@ def main() -> int:
         edp.zero_grad()
         loss = loss_of(edp)
         loss.backward()
-        edp.reduce_grads()
+        edp.reduce_grads(optimizer=opt if a.master_weights else None)
         opt.step()
         torch.cuda.synchronize()
         now = time.time()
