@@ -232,6 +232,34 @@ int tok_sgd_master_step(const tok_sgd_segment_t* segments, int count, int64_t ch
                         double lr, double momentum, double dampening, double weight_decay,
                         int nesterov, int fresh, void* cuda_stream);
 
+/* Adam / AdamW step on fp32 master weights for bf16 / f16 parameters (torch_on_k8s_b200/optim.py),
+ * one launch per gradient bucket and param group for the parameters that share a step count.  For
+ * every element of every segment it produces the bits of
+ *   torch.optim.Adam(masters, lr, (beta1, beta2), eps, weight_decay, amsgrad,
+ *                    decoupled_weight_decay).step()                                   (foreach)
+ *   param.copy_(master)                                                               (RNE)
+ * with grad = f32(segment.grad) as the master's gradient and `step` the parameters' step count after
+ * its increment (>= 1).  `decoupled` != 0 is AdamW's decay; `amsgrad` != 0 keeps max_exp_avg_sq.  The
+ * hyperparameters are torch's Python floats: the bias corrections are computed from them in double,
+ * as torch's Python does, and every scalar is rounded to float as ATen rounds it.  The table follows
+ * tok_sgd_master_step's rules (TOK_SGD_CHUNK elements per chunk, one CTA per chunk, a DEVICE array).
+ * Returns TOK_ERR_INVALID for an empty table, a dtype other than TOK_BF16 / TOK_F16, a negative or
+ * non-finite lr, eps or weight_decay, betas outside [0, 1) or a step below 1 or non-finite,
+ * TOK_ERR_NO_DEVICE without a GPU.  Enqueued on `cuda_stream`, no synchronisation. */
+typedef struct tok_adam_segment {
+  const void* grad;       /* bf16 / f16[numel], the parameter's gradient (anywhere in its bucket) */
+  void* param;            /* bf16 / f16[numel], written                                           */
+  float* master;          /* fp32[numel], read and written                                        */
+  float* exp_avg;         /* fp32[numel], read and written                                        */
+  float* exp_avg_sq;      /* fp32[numel], read and written                                        */
+  float* max_exp_avg_sq;  /* fp32[numel], read and written when amsgrad, else NULL                */
+  int64_t numel;
+  int64_t chunk0;         /* index of this segment's first chunk                                  */
+} tok_adam_segment_t;
+int tok_adam_master_step(const tok_adam_segment_t* segments, int count, int64_t chunks, int dtype,
+                         double lr, double beta1, double beta2, double eps, double weight_decay,
+                         int decoupled, int amsgrad, double step, void* cuda_stream);
+
 /* Which algorithm AUTO picks for `wire_bytes` on this communicator. */
 int tok_allreduce_algo(tok_comm_t* comm, size_t wire_bytes, int* algo);
 /* Number of kernels this communicator has launched so far (bench.py's gpu_launches): exchange,

@@ -39,6 +39,38 @@ def card():
     return dict(zip(q.split(","), [s.strip() for s in out.split(",")]))
 
 
+def timed(fn, k=50):
+    """Milliseconds per call of fn over k calls after 5 warm-up calls, by CUDA events."""
+    import torch
+    for _ in range(5):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(k):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / k
+
+
+def kernel_breakdown(prof, steps, optimizer_keys):
+    """Per-step device time of a torch.profiler run of `steps` steps: the step's kernel total, the
+    25 largest entries and the 12 largest whose names contain one of optimizer_keys."""
+    rows = []
+    for ev in prof.key_averages():
+        t = getattr(ev, "device_time_total", 0) or getattr(ev, "cuda_time_total", 0)
+        if t > 0:
+            rows.append((t / steps / 1e3, ev.count // steps, ev.key))
+    rows.sort(reverse=True)
+    opt_rows = [r for r in rows if any(s in r[2] for s in optimizer_keys)]
+    return dict(step_kernel_ms=sum(r[0] for r in rows if r[1] > 0),
+                top=[dict(ms_per_step=round(t, 4), launches_per_step=c, kernel=k[:120])
+                     for t, c, k in rows[:25]],
+                optimizer_like=[dict(ms_per_step=round(t, 4), launches_per_step=c, kernel=k[:120])
+                                for t, c, k in opt_rows[:12]])
+
+
 def main() -> int:
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=256)
@@ -141,20 +173,9 @@ def main() -> int:
                     arms[name]()
                 torch.cuda.synchronize()
             done[name] += 5
-            rows = []
-            for ev in prof.key_averages():
-                t = getattr(ev, "device_time_total", 0) or getattr(ev, "cuda_time_total", 0)
-                if t > 0:
-                    rows.append((t / 5 / 1e3, ev.count // 5, ev.key))
-            rows.sort(reverse=True)
-            opt_rows = [r for r in rows if any(s in r[2] for s in ("sgd_master", "foreach", "multi_tensor",
-                                                                   "copy", "to_copy", "Cast"))]
             emit(dict(base, kind="profile", arm=name, steps_profiled=5,
-                      step_kernel_ms=sum(r[0] for r in rows if r[1] > 0),
-                      top=[dict(ms_per_step=round(t, 4), launches_per_step=c, kernel=k[:120])
-                           for t, c, k in rows[:25]],
-                      optimizer_like=[dict(ms_per_step=round(t, 4), launches_per_step=c, kernel=k[:120])
-                                      for t, c, k in opt_rows[:12]]))
+                      **kernel_breakdown(prof, 5, ("sgd_master", "foreach", "multi_tensor", "copy",
+                                                   "to_copy", "Cast"))))
     else:
         for name, fn in arms.items():
             for _ in range(a.warmup):
@@ -202,17 +223,6 @@ def main() -> int:
         for p in p2:
             p.grad = torch.empty_like(p).normal_(0, 1e-3)
 
-        def timed(fn, k=50):
-            for _ in range(5):
-                fn()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(k):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            return e0.elapsed_time(e1) / k
         # the kernel alone: one launch over the table step() uploaded, without step()'s Python work
         import ctypes
         from torch_on_k8s_b200 import _ffi

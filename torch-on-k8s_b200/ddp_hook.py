@@ -24,9 +24,9 @@ class BucketAllreduceHook:
     overlaps the backward kernels that are still producing bucket k+1 (DDP's own overlap model);
     the returned CUDA-aware Future carries the event consumers must wait on.
 
-    optimizer (a MasterWeightSGD): each bucket's optimizer step is enqueued on the same stream right
-    behind its exchange, before the Future is set; optimizer.step() then only orders the current
-    stream after that stream.
+    optimizer (a MasterWeightSGD, MasterWeightAdam or MasterWeightAdamW): each bucket's optimizer
+    step is enqueued on the same stream right behind its exchange, before the Future is set;
+    optimizer.step() then only orders the current stream after that stream.
     """
 
     def __init__(self, comm: Communicator, *, wire_dtype: Optional[torch.dtype] = None,

@@ -90,8 +90,9 @@ class ElasticDataParallel(torch.nn.Module):
 
     def reduce_grads(self, stream: Optional[torch.cuda.Stream] = None, optimizer=None) -> None:
         """Average the gradient buckets across the current peer group (in place, zero-copy).
-        optimizer (a MasterWeightSGD): each bucket's step is enqueued right behind its exchange;
-        optimizer.step() then launches nothing for these parameters."""
+        optimizer (a MasterWeightSGD, MasterWeightAdam or MasterWeightAdamW): each bucket's step is
+        enqueued right behind its exchange; optimizer.step() then launches nothing for these
+        parameters."""
         world = self.comm.world
         for k, b in enumerate(self.buckets):   # PRE scale: the same function as built-in DDP
             self.comm.allreduce_bucket(b, b, scale=1.0 / world, algo=self.algo, stream=stream)

@@ -43,9 +43,9 @@ class Replica:
         path, with identical results.  A pool that cannot be created raises rather than change
         kernels silently: pass zero_copy=False to ask for the staged path.
 
-        optimizer (a torch_on_k8s_b200.optim.MasterWeightSGD over the model's parameters): the hook
-        steps each bucket's parameters right behind the bucket's exchange; optimizer.step() then
-        launches nothing for them."""
+        optimizer (a torch_on_k8s_b200.optim.MasterWeightSGD, MasterWeightAdam or MasterWeightAdamW
+        over the model's parameters): the hook steps each bucket's parameters right behind the
+        bucket's exchange; optimizer.step() then launches nothing for them."""
         from torch.nn.parallel import DistributedDataParallel as DDP
         pooled = zero_copy and self.world > 1 and wire_dtype is None
         if pooled:

@@ -37,7 +37,10 @@ def main() -> int:
     ap.add_argument("--log-every", type=int, default=10)
     ap.add_argument("--master-weights", action="store_true",
                     help="bf16 / f16 models: SGD on fp32 master weights, stepped behind each "
-                         "bucket's exchange (torch_on_k8s_b200.optim.MasterWeightSGD)")
+                         "bucket's exchange (torch_on_k8s_b200.optim.MasterWeightSGD, or "
+                         "MasterWeightAdamW with --optimizer adamw)")
+    ap.add_argument("--optimizer", choices=("sgd", "adamw"), default="sgd",
+                    help="sgd: lr 0.01, momentum 0.9; adamw: torch.optim.AdamW's defaults")
     a = ap.parse_args()
 
     import torch
@@ -50,12 +53,14 @@ def main() -> int:
     if len(shape) == 3:
         model = model.to(memory_format=torch.channels_last)
     if a.master_weights:
-        from torch_on_k8s_b200.optim import MasterWeightSGD
-        opt = MasterWeightSGD(model.parameters(), lr=0.01, momentum=0.9)
+        from torch_on_k8s_b200.optim import MasterWeightAdamW, MasterWeightSGD
+        opt = MasterWeightAdamW(model.parameters()) if a.optimizer == "adamw" else \
+            MasterWeightSGD(model.parameters(), lr=0.01, momentum=0.9)
         ddp, hook = rep.wrap(model, record_events=(rep.rank == 0), optimizer=opt)
     else:
         ddp, hook = rep.wrap(model, record_events=(rep.rank == 0))
-        opt = torch.optim.SGD(ddp.parameters(), lr=0.01, momentum=0.9)
+        opt = torch.optim.AdamW(ddp.parameters()) if a.optimizer == "adamw" else \
+            torch.optim.SGD(ddp.parameters(), lr=0.01, momentum=0.9)
     sampler = ReplicaSampler(a.steps * a.batch * rep.world, rep.world, rep.rank, seed=0)
     gen = torch.Generator(device=rep.device).manual_seed(1234 + rep.rank)
     t_prev = time.time()

@@ -59,7 +59,10 @@ def main() -> int:
     ap.add_argument("--log-every", type=int, default=5)
     ap.add_argument("--master-weights", action="store_true",
                     help="bf16 models: SGD on fp32 master weights, stepped behind each bucket's "
-                         "exchange (torch_on_k8s_b200.optim.MasterWeightSGD)")
+                         "exchange (torch_on_k8s_b200.optim.MasterWeightSGD, or MasterWeightAdamW "
+                         "with --optimizer adamw)")
+    ap.add_argument("--optimizer", choices=("sgd", "adamw"), default="sgd",
+                    help="sgd: momentum 0.9; adamw: torch.optim.AdamW's defaults but --lr")
     a = ap.parse_args()
 
     t_proc = time.time()
@@ -80,10 +83,12 @@ def main() -> int:
     name = os.environ.get("TOK8S_REPLICA", "replica-%d" % rep.rank)
     edp = ElasticDataParallel(model, rep.comm, bucket_cap_mb=25)
     if a.master_weights:
-        from torch_on_k8s_b200.optim import MasterWeightSGD
-        opt = MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9)
+        from torch_on_k8s_b200.optim import MasterWeightAdamW, MasterWeightSGD
+        opt = MasterWeightAdamW(model.parameters(), lr=a.lr) if a.optimizer == "adamw" else \
+            MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9)
     else:
-        opt = torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
+        opt = torch.optim.AdamW(model.parameters(), lr=a.lr) if a.optimizer == "adamw" else \
+            torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
     sampler = ReplicaSampler(a.steps * a.batch * 8, rep.world, rep.rank, seed=0)
 
     def log(**kw):
