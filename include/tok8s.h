@@ -205,6 +205,20 @@ int tok_bn2_add_relu_fwd(const void* x, const float* mean, const float* var, con
                          const void* bias_d, float eps_d, float* invstd_d, void* y, int64_t rows,
                          int channels, void* cuda_stream);
 
+/* Batch-norm batch statistics (training) of an NHWC bf16 activation seen as [rows = N*H*W, channels],
+ * bit-identical to torch.batch_norm_update_stats: writes the float batch mean and biased variance to
+ * `mean` and `var` (float[channels]) and updates the bf16 running statistics in place with
+ * `momentum` and the unbiased variance.  `workspace` holds tok_bn_stats_workspace_bytes(rows,
+ * channels) bytes (may be NULL when that is 0); it needs no initialisation.  The activation and the
+ * workspace must be 16-byte aligned and channels a multiple of 8 (TOK_ERR_ALIGN); rows * channels
+ * must stay below 2^31 (TOK_ERR_INVALID).  Enqueued on `cuda_stream` (two launches at most), no
+ * synchronisation; TOK_ERR_NO_DEVICE without a GPU.  tok_bn_stats_workspace_bytes returns the byte
+ * count, or a TOK_ERR_* code for a shape tok_bn_stats_fwd refuses. */
+int64_t tok_bn_stats_workspace_bytes(int64_t rows, int channels);
+int tok_bn_stats_fwd(const void* x, int64_t rows, int channels, double momentum, void* running_mean,
+                     void* running_var, void* workspace, float* mean, float* var,
+                     void* cuda_stream);
+
 /* SGD step on fp32 master weights for bf16 / f16 parameters (torch_on_k8s_b200/optim.py), one launch
  * per gradient bucket.  For every element of every segment it produces the bits of
  *   torch.optim.SGD(masters, lr, momentum, dampening, weight_decay, nesterov).step()   (foreach)

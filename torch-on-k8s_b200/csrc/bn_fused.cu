@@ -1,7 +1,9 @@
-// Batch-norm forward apply fused with ReLU and the residual add, NHWC bf16 (training).
+// Batch-norm forward, NHWC bf16 (training): the batch statistics, and the apply fused with ReLU and
+// the residual add.
 //
 // The activation of a channels_last [N, C, H, W] tensor is the row-major matrix [M = N*H*W, C].
-// The statistics (mean, biased variance) come from ATen's own channels_last statistics kernel; these
+// The statistics (mean, biased variance, running-statistics update) reproduce ATen's channels_last
+// statistics kernel and batch_norm_update_stats bit for bit (see "batch statistics" below); the apply
 // kernels replace the passes that follow it in stock PyTorch:
 //
 //   mode 0:  y = relu(bf16(T(x)))                                  bn -> relu_
@@ -24,6 +26,7 @@
 
 #include <atomic>
 
+#include "bn_stats_geom.h"
 #include "tok_internal.h"
 
 namespace tok {
@@ -149,6 +152,221 @@ __global__ void __launch_bounds__(kBnThreads) bn_fused_fwd_kernel(const BnArgs p
   }
 }
 
+// ---- batch statistics ---------------------------------------------------------------------------
+// The arithmetic of ATen's batch_norm_collect_statistics_channels_last_kernel<Var, BFloat16, float, 4>
+// and of the update lambda of batch_norm_update_stats, pinned op by op as the sm_90 code of torch's
+// libtorch_cuda.so performs it (cuobjdump -sass):
+//   step      d0 = x - mean; mean = fma(d0, inv, mean); d1 = x - mean; m2 = fma(d0 * d1, valid, m2)
+//             with inv = 1 / count correctly rounded (valid slot) or x = inv = valid = 0 (a slot past
+//             the last row, still executed: it turns an infinite mean into NaN)
+//   merge     f = 1 / max(1, n + nb) correctly rounded; d = mean - mean_b;
+//             m2 = m2 + fma(((d * d) * nb) * n, f, m2_b); n += nb; and the mean
+//             j-merge:   mean = fma(mean_b, nb, mean * n) * f     (chains 1, 2, 3 into chain 0)
+//             tree/grid: mean = fma(mean, n, mean_b * nb) * f     (every other merge)
+//   finish    var = m2 / n (IEEE division)
+//   running   r_mean = bf16(fma(mean, momentum, (1 - momentum) * r_mean))
+//             r_var  = bf16(fma(var * bessel, momentum, (1 - momentum) * r_var))
+// The geometry is bn_stats_geom.h's.  Logical thread (by, ty) of ATen becomes one thread per 8-channel
+// vector here; its 4 chains visit rows p + (4i + j) * P (p = by * block_y + ty, P = block_y * grid_y).
+struct StatsArgs {
+  const uint4* x;
+  int* ws_count;   // grid_y > 1: per logical block partials, merged by the finish kernel
+  float* ws_mean;
+  float* ws_m2;
+  float* mean;
+  float* var;
+  __nv_bfloat16* running_mean;
+  __nv_bfloat16* running_var;
+  int rows;
+  int channels;
+  int vecs;
+  int block_y;
+  int grid_y;
+  int loop_count;
+  float momentum;
+  float bessel;
+};
+
+constexpr int kStatsThreads = 256;  // physical threads per block of the finish kernel
+// Physical threads per block of the partial kernel.  At ~160 registers a thread, 128-thread blocks
+// let 3 blocks share an SM, and they split the 128 logical blocks of a 64-channel site over 128
+// SMs rather than fewer.
+constexpr int kStatsPartialThreads = 128;
+constexpr int kStatsDepth = 2;      // iterations (of 4 rows) loaded ahead of the one computed
+
+// Folds (nb, mean_b, m2_b) into (n, mean, m2); the caller then adds nb to n (one count serves the
+// 8 channels of a vector).
+template <bool kJMerge>
+__device__ __forceinline__ void welford_merge(int n, float& mean, float& m2, int nb, float mean_b,
+                                              float m2_b) {
+  const float f = __frcp_rn(__int2float_rn(max(1, n + nb)));
+  const float fn = __int2float_rn(n), fnb = __int2float_rn(nb);
+  const float d = __fsub_rn(mean, mean_b);
+  mean = kJMerge ? __fmul_rn(__fmaf_rn(mean_b, fnb, __fmul_rn(mean, fn)), f)
+                 : __fmul_rn(__fmaf_rn(mean, fn, __fmul_rn(mean_b, fnb)), f);
+  m2 = __fadd_rn(m2, __fmaf_rn(__fmul_rn(__fmul_rn(__fmul_rn(d, d), fnb), fn), f, m2_b));
+}
+
+__device__ __forceinline__ void stats_finish(const StatsArgs& a, int c, int n, float mean, float m2) {
+  const float var = __fdiv_rn(m2, __int2float_rn(n));
+  a.mean[c] = mean;
+  a.var[c] = var;
+  const float keep = __fsub_rn(1.0f, a.momentum);
+  const float rm = __bfloat162float(a.running_mean[c]);
+  const float rv = __bfloat162float(a.running_var[c]);
+  a.running_mean[c] = __float2bfloat16_rn(__fmaf_rn(mean, a.momentum, __fmul_rn(keep, rm)));
+  a.running_var[c] =
+      __float2bfloat16_rn(__fmaf_rn(__fmul_rn(var, a.bessel), a.momentum, __fmul_rn(keep, rv)));
+}
+
+__device__ __forceinline__ void load_rows(const StatsArgs& a, int v, int64_t row, int64_t stride,
+                                          uint4 (&q)[kStatsChains]) {
+#pragma unroll
+  for (int j = 0; j < kStatsChains; ++j) {
+    const int64_t r = row + j * stride;
+    q[j] = r < a.rows ? __ldg(a.x + r * a.vecs + v) : make_uint4(0, 0, 0, 0);
+  }
+}
+
+// blockDim = (tile, block_y): thread (vx, ty) of block (bx, by) owns vector bx * tile + vx of
+// logical thread (by, ty).
+__global__ void __launch_bounds__(kStatsPartialThreads) bn_stats_partial_kernel(const StatsArgs a) {
+  __shared__ float s_mean[kStatsPartialThreads][kVec];
+  __shared__ float s_m2[kStatsPartialThreads][kVec];
+  __shared__ int s_n[kStatsPartialThreads];
+  const int tile = blockDim.x, ty = threadIdx.y;
+  const int v = blockIdx.x * tile + threadIdx.x;
+  const bool live = v < a.vecs;
+  const int64_t stride = (int64_t)a.block_y * a.grid_y;
+  const int64_t p = (int64_t)blockIdx.y * a.block_y + ty;
+
+  float mean[kStatsChains][kVec], m2[kStatsChains][kVec];
+  int n[kStatsChains];
+#pragma unroll
+  for (int j = 0; j < kStatsChains; ++j) {
+    n[j] = 0;
+#pragma unroll
+    for (int k = 0; k < kVec; ++k) mean[j][k] = m2[j][k] = 0.0f;
+  }
+
+  if (live) {
+    uint4 buf[kStatsDepth][kStatsChains];
+#pragma unroll
+    for (int s = 0; s < kStatsDepth; ++s)
+      load_rows(a, v, p + (int64_t)s * kStatsChains * stride, stride, buf[s]);
+    for (int i0 = 0; i0 < a.loop_count; i0 += kStatsDepth) {
+#pragma unroll
+      for (int s = 0; s < kStatsDepth; ++s) {
+        const int i = i0 + s;
+        if (i < a.loop_count) {
+          const int64_t row = p + (int64_t)i * kStatsChains * stride;
+          uint4 next[kStatsChains];
+          load_rows(a, v, row + (int64_t)kStatsDepth * kStatsChains * stride, stride, next);
+          // A chain's valid slots are a prefix of its iterations, so a valid slot of iteration i
+          // has count i + 1: one correctly rounded 1 / count serves 4 chains of 8 channels.
+          const float inv_i = __frcp_rn(__int2float_rn(i + 1));
+#pragma unroll
+          for (int j = 0; j < kStatsChains; ++j) {
+            const bool valid = row + j * stride < a.rows;
+            if (valid) ++n[j];
+            const float inv = valid ? inv_i : 0.0f;
+            const float vf = valid ? 1.0f : 0.0f;
+#pragma unroll
+            for (int k = 0; k < kVec; ++k) {
+              const float x = widen(word(buf[s][j], k >> 1), k & 1);
+              const float d0 = __fsub_rn(x, mean[j][k]);
+              mean[j][k] = __fmaf_rn(d0, inv, mean[j][k]);
+              const float d1 = __fsub_rn(x, mean[j][k]);
+              m2[j][k] = __fmaf_rn(__fmul_rn(d0, d1), vf, m2[j][k]);
+            }
+            buf[s][j] = next[j];
+          }
+        }
+      }
+    }
+  }
+
+#pragma unroll
+  for (int j = 1; j < kStatsChains; ++j) {
+#pragma unroll
+    for (int k = 0; k < kVec; ++k)
+      welford_merge<true>(n[0], mean[0][k], m2[0][k], n[j], mean[j][k], m2[j][k]);
+    n[0] += n[j];
+  }
+
+  // ATen's welford_merge_block_vertical over ty
+  const int slot = ty * tile + threadIdx.x;
+  for (int off = a.block_y / 2; off > 0; off >>= 1) {
+    if (ty < 2 * off) {
+#pragma unroll
+      for (int k = 0; k < kVec; ++k) {
+        s_mean[slot][k] = mean[0][k];
+        s_m2[slot][k] = m2[0][k];
+      }
+      s_n[slot] = n[0];
+    }
+    __syncthreads();
+    if (ty < off) {
+      const int o = slot + off * tile;
+      const int nb = s_n[o];
+#pragma unroll
+      for (int k = 0; k < kVec; ++k)
+        welford_merge<false>(n[0], mean[0][k], m2[0][k], nb, s_mean[o][k], s_m2[o][k]);
+      n[0] += nb;
+    }
+    __syncthreads();
+  }
+  if (ty != 0 || !live) return;
+  if (a.grid_y == 1) {
+#pragma unroll
+    for (int k = 0; k < kVec; ++k) stats_finish(a, v * kVec + k, n[0], mean[0][k], m2[0][k]);
+    return;
+  }
+  const int64_t base = (int64_t)blockIdx.y * a.channels + v * kVec;
+#pragma unroll
+  for (int k = 0; k < kVec; ++k) {
+    a.ws_mean[base + k] = mean[0][k];
+    a.ws_m2[base + k] = m2[0][k];
+  }
+  if (v == 0) a.ws_count[blockIdx.y] = n[0];
+}
+
+// ATen's last-block merge: blockDim = (kStatsThreads / block_y, block_y), one channel per column.
+// Lane ty folds logical blocks ty, ty + block_y, ... into the zero state, then the vertical tree.
+__global__ void __launch_bounds__(kStatsThreads) bn_stats_finish_kernel(const StatsArgs a) {
+  __shared__ float s_mean[kStatsThreads], s_m2[kStatsThreads];
+  __shared__ int s_n[kStatsThreads];
+  const int cols = blockDim.x, ty = threadIdx.y;
+  const int c = blockIdx.x * cols + threadIdx.x;
+  const bool live = c < a.channels;
+  int n = 0;
+  float mean = 0.0f, m2 = 0.0f;
+  if (live) {
+    for (int y = ty; y < a.grid_y; y += a.block_y) {
+      const int64_t o = (int64_t)y * a.channels + c;
+      const int nb = a.ws_count[y];
+      welford_merge<false>(n, mean, m2, nb, a.ws_mean[o], a.ws_m2[o]);
+      n += nb;
+    }
+  }
+  const int slot = ty * cols + threadIdx.x;
+  for (int off = a.block_y / 2; off > 0; off >>= 1) {
+    if (ty < 2 * off) {
+      s_mean[slot] = mean;
+      s_m2[slot] = m2;
+      s_n[slot] = n;
+    }
+    __syncthreads();
+    if (ty < off) {
+      const int o = slot + off * cols;
+      welford_merge<false>(n, mean, m2, s_n[o], s_mean[o], s_m2[o]);
+      n += s_n[o];
+    }
+    __syncthreads();
+  }
+  if (ty == 0 && live) stats_finish(a, c, n, mean, m2);
+}
+
 }  // namespace
 
 // ---- host side --------------------------------------------------------------------------------
@@ -230,6 +448,18 @@ BnSide side(const void* x, const float* mean, const float* var, const void* weig
                 (const __nv_bfloat16*)bias, invstd, eps};
 }
 
+int check_stats_shape(const char* who, int64_t rows, int channels) {
+  if (rows <= 0 || channels <= 0)
+    return fail(TOK_ERR_INVALID, "%s: rows %lld and channels %d must be positive", who,
+                (long long)rows, channels);
+  if (rows * channels > INT32_MAX)
+    return fail(TOK_ERR_INVALID, "%s: %lld x %d elements exceed 32-bit indexing", who,
+                (long long)rows, channels);
+  if (channels % kVec != 0)
+    return fail(TOK_ERR_ALIGN, "%s: channels %d is not a multiple of %d", who, channels, kVec);
+  return TOK_OK;
+}
+
 }  // namespace
 }  // namespace tok
 
@@ -287,4 +517,68 @@ extern "C" int tok_bn2_add_relu_fwd(const void* x, const float* mean, const floa
   a.rows = rows;
   a.vecs = channels / kVec;
   return launch<2>(a, cuda_stream);
+}
+
+extern "C" int64_t tok_bn_stats_workspace_bytes(int64_t rows, int channels) {
+  const int rc = check_stats_shape("tok_bn_stats_workspace_bytes", rows, channels);
+  if (rc != TOK_OK) return rc;
+  return bn_stats_workspace(bn_stats_geometry((int)rows, channels), channels);
+}
+
+extern "C" int tok_bn_stats_fwd(const void* x, int64_t rows, int channels, double momentum,
+                                void* running_mean, void* running_var, void* workspace,
+                                float* mean, float* var, void* cuda_stream) {
+  const char* who = "tok_bn_stats_fwd";
+  if (!x || !running_mean || !running_var || !mean || !var)
+    return fail(TOK_ERR_INVALID, "%s: null pointer argument", who);
+  int rc = check_stats_shape(who, rows, channels);
+  if (rc != TOK_OK) return rc;
+  if (misaligned(x)) return fail(TOK_ERR_ALIGN, "%s: activation is not 16-byte aligned", who);
+  const BnStatsGeom g = bn_stats_geometry((int)rows, channels);
+  const int64_t ws_bytes = bn_stats_workspace(g, channels);
+  if (ws_bytes > 0 && !workspace)
+    return fail(TOK_ERR_INVALID, "%s: null workspace (%lld bytes needed)", who, (long long)ws_bytes);
+  if (ws_bytes > 0 && misaligned(workspace))
+    return fail(TOK_ERR_ALIGN, "%s: workspace is not 16-byte aligned", who);
+  if (!device_ready()) return fail(TOK_ERR_NO_DEVICE, "%s needs a CUDA GPU (no CPU fallback)", who);
+
+  StatsArgs a{};
+  a.x = (const uint4*)x;
+  if (ws_bytes > 0) {
+    const int64_t counts = ws_bytes - 2 * (int64_t)g.grid_y * channels * 4;
+    a.ws_count = (int*)workspace;
+    a.ws_mean = (float*)((char*)workspace + counts);
+    a.ws_m2 = a.ws_mean + (int64_t)g.grid_y * channels;
+  }
+  a.mean = mean;
+  a.var = var;
+  a.running_mean = (__nv_bfloat16*)running_mean;
+  a.running_var = (__nv_bfloat16*)running_var;
+  a.rows = (int)rows;
+  a.channels = channels;
+  a.vecs = channels / kVec;
+  a.block_y = g.block_y;
+  a.grid_y = g.grid_y;
+  a.loop_count = g.loop_count;
+  // as ATen's batch_norm_update_stats: float(momentum), float(N / (N - 1)) formed in double
+  a.momentum = (float)momentum;
+  a.bessel = (float)((double)rows / (double)(rows - 1));
+
+  // the partial kernel: block (tile, block_y), one 8-channel vector per thread
+  int tile = kStatsPartialThreads / g.block_y;
+  if (tile > a.vecs) tile = a.vecs;
+  const dim3 block(tile, g.block_y);
+  const dim3 grid((a.vecs + tile - 1) / tile, g.grid_y);
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  bn_stats_partial_kernel<<<grid, block, 0, st>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(TOK_ERR_CUDA, "bn_stats_partial launch: %s", cudaGetErrorString(e));
+  if (g.grid_y > 1) {
+    const int cols = kStatsThreads / g.block_y;
+    bn_stats_finish_kernel<<<(channels + cols - 1) / cols, dim3(cols, g.block_y), 0, st>>>(a);
+    e = cudaGetLastError();
+    if (e != cudaSuccess)
+      return fail(TOK_ERR_CUDA, "bn_stats_finish launch: %s", cudaGetErrorString(e));
+  }
+  return TOK_OK;
 }

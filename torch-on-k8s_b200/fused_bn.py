@@ -9,11 +9,12 @@ gradients, their running statistics and `num_batches_tracked` are updated exactl
 forward would update them.  The results, the gradients and the updated buffers are bit-identical to
 the unfused composition, so swapping these in changes no number of a training run.
 
-What is fused: the forward elementwise passes.  The batch statistics still come from ATen's
-channels_last statistics kernel (`torch.batch_norm_update_stats`, which also updates the running
-statistics); one libtok8s kernel then applies the normalisation with ATen's exact float expression,
-adds the residual (or the second, downsample batch norm) and applies the ReLU, writing one bf16
-tensor where the stock composition writes and re-reads two or three.  The backward is the stock
+What is fused: the forward passes.  The batch statistics and the running-statistics update come
+from libtok8s's statistics kernels, which perform the arithmetic of ATen's channels_last statistics
+kernel and of `torch.batch_norm_update_stats` in the same order, bit for bit, with 16-byte loads
+and more loads in flight; one libtok8s kernel then applies the normalisation with ATen's exact
+float expression, adds the residual (or the second, downsample batch norm) and applies the ReLU,
+writing one bf16 tensor where the stock composition writes and re-reads two or three.  The backward is the stock
 one: `threshold_backward` on the saved output, then `native_batch_norm_backward` with the saved
 mean and invstd, saving the same activations stock autograd saves (the batch-norm inputs and the
 ReLU output).
@@ -58,10 +59,24 @@ def _same(a: torch.Tensor, b: torch.Tensor) -> bool:
 
 
 def _stats(x: torch.Tensor, bn: torch.nn.Module):
-    """Batch mean and biased variance (float) from ATen's channels_last statistics kernel, with the
+    """Batch mean and biased variance (float), bit-identical to torch.batch_norm_update_stats, with the
     running statistics and num_batches_tracked updated as nn.BatchNorm2d.forward updates them."""
     bn.num_batches_tracked.add_(1)
-    return torch.batch_norm_update_stats(x, bn.running_mean, bn.running_var, bn.momentum)
+    rows, ch = x.numel() // x.shape[1], x.shape[1]
+    lib = _ffi.lib()
+    nbytes = lib.tok_bn_stats_workspace_bytes(rows, ch)
+    if nbytes < 0:
+        _ffi.check(nbytes)
+    mean = torch.empty(ch, dtype=torch.float32, device=x.device)
+    var = torch.empty_like(mean)
+    work = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    with torch.cuda.device(x.device):
+        stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
+        rc = lib.tok_bn_stats_fwd(_ptr(x), rows, ch, bn.momentum, _ptr(bn.running_mean),
+                                  _ptr(bn.running_var), _ptr(work) if nbytes else None, _ptr(mean),
+                                  _ptr(var), stream)
+    _ffi.check(rc)
+    return mean, var
 
 
 def _ptr(t):
