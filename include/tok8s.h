@@ -219,6 +219,33 @@ int tok_bn_stats_fwd(const void* x, int64_t rows, int channels, double momentum,
                      void* running_var, void* workspace, float* mean, float* var,
                      void* cuda_stream);
 
+/* Batch-norm backward (training) with the ReLU backward folded in, one entry point per forward above,
+ * bit-identical to threshold_backward(gy, y, 0) followed by native_batch_norm_backward with the saved
+ * `mean` and `invstd` (float[channels]).  The ReLU mask is (v <= 0 ? 0 : gy): in tok_bn_relu_bwd v is
+ * bf16(bn(x)) recomputed from x, mean, invstd, weight and bias; otherwise v is the saved output y,
+ * and the masked gradient is written to `dz` (the residual's gradient; for tok_bn2_add_relu_bwd a
+ * scratch tensor).  dx / dxd, grad_weight and grad_bias (bf16) are written where not NULL; with no
+ * dx (and no dxd) only the reduction runs.  `workspace` holds tok_bn_bwd_workspace_bytes(rows,
+ * channels, mode) bytes, mode 0, 1, 2 as the three entry points; it needs no initialisation.
+ * Activations and the workspace must be 16-byte aligned and channels a multiple of 8
+ * (TOK_ERR_ALIGN); rows * channels must stay below 2^31 (TOK_ERR_INVALID).  Enqueued on
+ * `cuda_stream` (three launches at most), no synchronisation; TOK_ERR_NO_DEVICE without a GPU.
+ * tok_bn_bwd_workspace_bytes returns the byte count, or a TOK_ERR_* code for a refused shape. */
+int64_t tok_bn_bwd_workspace_bytes(int64_t rows, int channels, int mode);
+int tok_bn_relu_bwd(const void* gy, const void* x, const float* mean, const float* invstd,
+                    const void* weight, const void* bias, void* dx, void* grad_weight,
+                    void* grad_bias, int64_t rows, int channels, void* workspace, void* cuda_stream);
+int tok_bn_add_relu_bwd(const void* gy, const void* y, const void* x, const float* mean,
+                        const float* invstd, const void* weight, void* dz, void* dx,
+                        void* grad_weight, void* grad_bias, int64_t rows, int channels,
+                        void* workspace, void* cuda_stream);
+int tok_bn2_add_relu_bwd(const void* gy, const void* y, const void* x, const float* mean,
+                         const float* invstd, const void* weight, const void* xd,
+                         const float* mean_d, const float* invstd_d, const void* weight_d, void* dz,
+                         void* dx, void* grad_weight, void* grad_bias, void* dxd,
+                         void* grad_weight_d, void* grad_bias_d, int64_t rows, int channels,
+                         void* workspace, void* cuda_stream);
+
 /* SGD step on fp32 master weights for bf16 / f16 parameters (torch_on_k8s_b200/optim.py), one launch
  * per gradient bucket.  For every element of every segment it produces the bits of
  *   torch.optim.SGD(masters, lr, momentum, dampening, weight_decay, nesterov).step()   (foreach)

@@ -114,6 +114,10 @@ PROTOTYPES = {
                                        C.c_float, _P, _P, C.c_int64, C.c_int, _P]),
     "tok_bn_stats_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int]),
     "tok_bn_stats_fwd": (C.c_int, [_P, C.c_int64, C.c_int, C.c_double, _P, _P, _P, _P, _P, _P]),
+    "tok_bn_bwd_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int, C.c_int]),
+    "tok_bn_relu_bwd": (C.c_int, [_P] * 9 + [C.c_int64, C.c_int, _P, _P]),
+    "tok_bn_add_relu_bwd": (C.c_int, [_P] * 10 + [C.c_int64, C.c_int, _P, _P]),
+    "tok_bn2_add_relu_bwd": (C.c_int, [_P] * 17 + [C.c_int64, C.c_int, _P, _P]),
     "tok_sgd_master_step": (C.c_int, [_P, C.c_int, C.c_int64, C.c_int, C.c_double, C.c_double,
                                       C.c_double, C.c_double, C.c_int, C.c_int, _P]),
     "tok_adam_master_step": (C.c_int, [_P, C.c_int, C.c_int64, C.c_int, C.c_double, C.c_double,

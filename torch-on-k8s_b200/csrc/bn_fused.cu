@@ -367,6 +367,331 @@ __global__ void __launch_bounds__(kStatsThreads) bn_stats_finish_kernel(const St
   if (ty == 0 && live) stats_finish(a, c, n, mean, m2);
 }
 
+// ---- backward ---------------------------------------------------------------------------------
+// threshold_backward(gy, y, 0) and native_batch_norm_backward in one reduction and one elementwise
+// pass.  The mask is threshold_backward's: dz = (v <= 0) ? +0 : gy, so a NaN v passes gy and ±0 masks.
+// The arithmetic is that of ATen's batch_norm_backward_reduce_channels_last_kernel<4, BFloat16, float,
+// BFloat16> and batch_norm_backward_elemt_channels_last_kernel, pinned as the sm_90 code of torch's
+// libtorch_cuda.so performs it (cuobjdump -sass):
+//   reduce    sum_dy = sum_dy + dz; sum_dy_xmu = fma(x - mean, dz, sum_dy_xmu), per chain; a slot
+//             past the last row is still executed with dz = x = 0 (an infinite mean makes it NaN)
+//   merges    plain float adds: chains 1, 2, 3 into chain 0 in order, then ATen's
+//             merge_block_vertical_backward tree, then the grid merge (lane ty adds logical blocks
+//             ty, ty + block_y, ... to 0.0, then the tree again)
+//   finish    grad_bias = bf16(sum_dy); grad_weight = bf16(sum_dy_xmu * invstd)
+//   elemt     dx = bf16(fma(-f1, x - mean, fma(-sum_dy, n, dz)) * f2), with per channel
+//             f1 = ((invstd * invstd) * sum_dy_xmu) * n and f2 = weight * invstd, and n = float(1.0 / M)
+//             formed in double on the host (ATen passes it as a kernel argument)
+// The logical geometry is bn_stats_geom.h's (ATen launches the reduction with the same coop
+// configuration).  Physically, the 4 chains of a logical thread run on 4 adjacent lanes, one chain
+// per lane on an 8-channel vector; lane 0 then adds lanes 1, 2, 3 in order.  That gives the
+// 64-channel sites 4x the threads a chain-per-thread mapping has.
+struct BwdSide {
+  const uint4* x;
+  const float* mean;
+  const float* invstd;
+  const __nv_bfloat16* weight;
+  float* sum_xmu;                  // float[channels]: the reduction's sum_dy_xmu
+  float* ws_xmu;                   // grid_y > 1: float[grid_y][channels] partials
+  __nv_bfloat16* grad_weight;      // may be null
+  __nv_bfloat16* grad_bias;        // may be null
+  uint4* dx;                       // may be null
+};
+
+struct BwdArgs {
+  BwdSide a;                       // the main batch norm
+  BwdSide d;                       // mode 2: the downsample batch norm
+  const uint4* gy;
+  const uint4* y;                  // modes 1, 2: the saved output, the mask's v
+  uint4* dz;                       // modes 1, 2: the masked gradient, written by the reduction
+  const __nv_bfloat16* bias;       // mode 0: for the recomputed v
+  float* sum_dy;                   // float[channels]
+  float* ws_dy;                    // grid_y > 1: float[grid_y][channels] partials
+  float norm;                      // float(1.0 / rows)
+  int rows;
+  int channels;
+  int vecs;
+  int block_y;
+  int grid_y;
+  int loop_count;
+};
+
+constexpr int kBwdPartialThreads = 512;  // physical threads per block of the reduction
+// chain steps loaded ahead of the one computed (mode 2 loads four streams a step)
+template <int kMode>
+constexpr int kBwdDepth = kMode == 2 ? 2 : 4;
+
+__device__ __forceinline__ float relu_grad(float g, float v) { return v <= 0.0f ? 0.0f : g; }
+
+__device__ __forceinline__ void load_bwd_column(const BwdSide& s, const __nv_bfloat16* bias, int v,
+                                                Column& c) {
+#pragma unroll
+  for (int k = 0; k < kVec; ++k) {
+    const int ch = v * kVec + k;
+    c.mean[k] = s.mean[ch];
+    c.inv[k] = s.invstd[ch];
+    c.w[k] = __bfloat162float(s.weight[ch]);
+    c.b[k] = bias ? __bfloat162float(bias[ch]) : 0.0f;
+  }
+}
+
+// q = {gy, x, y, xd} of row r, zeros past the last row
+template <int kMode>
+__device__ __forceinline__ void load_bwd_row(const BwdArgs& a, int v, int64_t r, uint4 (&q)[4]) {
+  const uint4 zero = make_uint4(0, 0, 0, 0);
+  q[0] = q[1] = q[2] = q[3] = zero;
+  if (r < a.rows) {
+    const int64_t i = r * a.vecs + v;
+    q[0] = __ldg(a.gy + i);
+    q[1] = __ldg(a.a.x + i);
+    if (kMode != 0) q[2] = __ldg(a.y + i);
+    if (kMode == 2) q[3] = __ldg(a.d.x + i);
+  }
+}
+
+template <int kMode>
+__device__ __forceinline__ void bwd_finish(const BwdArgs& a, int c, float dy, float xmu,
+                                           float xmu_d) {
+  a.sum_dy[c] = dy;
+  a.a.sum_xmu[c] = xmu;
+  if (a.a.grad_bias) a.a.grad_bias[c] = __float2bfloat16_rn(dy);
+  if (a.a.grad_weight) a.a.grad_weight[c] = __float2bfloat16_rn(__fmul_rn(xmu, a.a.invstd[c]));
+  if (kMode == 2) {
+    a.d.sum_xmu[c] = xmu_d;
+    if (a.d.grad_bias) a.d.grad_bias[c] = __float2bfloat16_rn(dy);
+    if (a.d.grad_weight) a.d.grad_weight[c] = __float2bfloat16_rn(__fmul_rn(xmu_d, a.d.invstd[c]));
+  }
+}
+
+// blockDim = (4 * tile, block_y): lane j = threadIdx.x % 4 of thread (vx = threadIdx.x / 4, ty) of
+// block (bx, by) runs chain j of logical thread (by, ty) on vector bx * tile + vx.
+template <int kMode>
+__global__ void __launch_bounds__(kBwdPartialThreads) bn_bwd_partial_kernel(const BwdArgs a) {
+  constexpr int kSlots = kBwdPartialThreads / kStatsChains;
+  __shared__ float s_dy[kSlots][kVec];
+  __shared__ float s_xmu[kSlots][kVec];
+  __shared__ float s_xmu_d[kMode == 2 ? kSlots : 1][kVec];
+  const int j = threadIdx.x % kStatsChains, tile = blockDim.x / kStatsChains, ty = threadIdx.y;
+  const int vx = threadIdx.x / kStatsChains;
+  const int v = blockIdx.x * tile + vx;
+  const bool live = v < a.vecs;
+  const int64_t stride = (int64_t)a.block_y * a.grid_y;
+  const int64_t step = kStatsChains * stride;
+  const int64_t p = (int64_t)blockIdx.y * a.block_y + ty + j * stride;
+
+  float dy[kVec], xmu[kVec], xmu_d[kVec];
+#pragma unroll
+  for (int k = 0; k < kVec; ++k) dy[k] = xmu[k] = xmu_d[k] = 0.0f;
+
+  if (live) {
+    Column ca, cd;
+    load_bwd_column(a.a, kMode == 0 ? a.bias : nullptr, v, ca);
+    if (kMode == 2) load_bwd_column(a.d, nullptr, v, cd);
+    uint4 buf[kBwdDepth<kMode>][4];
+#pragma unroll
+    for (int s = 0; s < kBwdDepth<kMode>; ++s) load_bwd_row<kMode>(a, v, p + s * step, buf[s]);
+    for (int i0 = 0; i0 < a.loop_count; i0 += kBwdDepth<kMode>) {
+#pragma unroll
+      for (int s = 0; s < kBwdDepth<kMode>; ++s) {
+        if (i0 + s < a.loop_count) {
+          const int64_t row = p + (int64_t)(i0 + s) * step;
+          uint4 q[4];
+#pragma unroll
+          for (int t = 0; t < 4; ++t) q[t] = buf[s][t];
+          load_bwd_row<kMode>(a, v, row + kBwdDepth<kMode> * step, buf[s]);
+          uint32_t dz_bits[4];
+#pragma unroll
+          for (int k = 0; k < kVec; ++k) {
+            const int w = k >> 1, h = k & 1;
+            const float x = widen(word(q[1], w), h);
+            const float v_mask = kMode == 0 ? bn_apply(x, ca, k) : widen(word(q[2], w), h);
+            const float dz = relu_grad(widen(word(q[0], w), h), v_mask);
+            dy[k] = __fadd_rn(dy[k], dz);
+            xmu[k] = __fmaf_rn(__fsub_rn(x, ca.mean[k]), dz, xmu[k]);
+            if (kMode == 2)
+              xmu_d[k] = __fmaf_rn(__fsub_rn(widen(word(q[3], w), h), cd.mean[k]), dz, xmu_d[k]);
+            const uint32_t b = __float_as_uint(dz) >> 16;
+            dz_bits[w] = h ? (dz_bits[w] | (b << 16)) : b;
+          }
+          if (kMode != 0 && row < a.rows)
+            a.dz[row * a.vecs + v] = make_uint4(dz_bits[0], dz_bits[1], dz_bits[2], dz_bits[3]);
+        }
+      }
+    }
+  }
+
+  // chains 1, 2, 3 into chain 0, in order
+  const int tid = threadIdx.y * blockDim.x + threadIdx.x;
+  const int nthreads = blockDim.x * blockDim.y;
+  const int lanes = min(32, nthreads - (tid & ~31));
+  const unsigned mask = lanes == 32 ? 0xffffffffu : (1u << lanes) - 1u;
+#pragma unroll
+  for (int k = 0; k < kVec; ++k) {
+    float o[kStatsChains], od[kStatsChains], odd[kStatsChains];
+#pragma unroll
+    for (int c = 1; c < kStatsChains; ++c) {
+      o[c] = __shfl_sync(mask, dy[k], c, kStatsChains);
+      od[c] = __shfl_sync(mask, xmu[k], c, kStatsChains);
+      if (kMode == 2) odd[c] = __shfl_sync(mask, xmu_d[k], c, kStatsChains);
+    }
+#pragma unroll
+    for (int c = 1; c < kStatsChains; ++c) {
+      dy[k] = __fadd_rn(dy[k], o[c]);
+      xmu[k] = __fadd_rn(xmu[k], od[c]);
+      if (kMode == 2) xmu_d[k] = __fadd_rn(xmu_d[k], odd[c]);
+    }
+  }
+
+  // ATen's merge_block_vertical_backward over ty, lane 0 of each chain group
+  const int slot = ty * tile + vx;
+  for (int off = a.block_y / 2; off > 0; off >>= 1) {
+    if (j == 0 && ty < 2 * off) {
+#pragma unroll
+      for (int k = 0; k < kVec; ++k) {
+        s_dy[slot][k] = dy[k];
+        s_xmu[slot][k] = xmu[k];
+        if (kMode == 2) s_xmu_d[slot][k] = xmu_d[k];
+      }
+    }
+    __syncthreads();
+    if (j == 0 && ty < off) {
+      const int o = slot + off * tile;
+#pragma unroll
+      for (int k = 0; k < kVec; ++k) {
+        dy[k] = __fadd_rn(dy[k], s_dy[o][k]);
+        xmu[k] = __fadd_rn(xmu[k], s_xmu[o][k]);
+        if (kMode == 2) xmu_d[k] = __fadd_rn(xmu_d[k], s_xmu_d[o][k]);
+      }
+    }
+    __syncthreads();
+  }
+  if (j != 0 || ty != 0 || !live) return;
+  if (a.grid_y == 1) {
+#pragma unroll
+    for (int k = 0; k < kVec; ++k) bwd_finish<kMode>(a, v * kVec + k, dy[k], xmu[k], xmu_d[k]);
+    return;
+  }
+  const int64_t base = (int64_t)blockIdx.y * a.channels + v * kVec;
+#pragma unroll
+  for (int k = 0; k < kVec; ++k) {
+    a.ws_dy[base + k] = dy[k];
+    a.a.ws_xmu[base + k] = xmu[k];
+    if (kMode == 2) a.d.ws_xmu[base + k] = xmu_d[k];
+  }
+}
+
+// ATen's last-block merge: blockDim = (kStatsThreads / block_y, block_y), one channel per column.
+template <int kMode>
+__global__ void __launch_bounds__(kStatsThreads) bn_bwd_finish_kernel(const BwdArgs a) {
+  __shared__ float s_dy[kStatsThreads], s_xmu[kStatsThreads];
+  __shared__ float s_xmu_d[kMode == 2 ? kStatsThreads : 1];
+  const int cols = blockDim.x, ty = threadIdx.y;
+  const int c = blockIdx.x * cols + threadIdx.x;
+  const bool live = c < a.channels;
+  float dy = 0.0f, xmu = 0.0f, xmu_d = 0.0f;
+  if (live) {
+    for (int y = ty; y < a.grid_y; y += a.block_y) {
+      const int64_t o = (int64_t)y * a.channels + c;
+      dy = __fadd_rn(dy, a.ws_dy[o]);
+      xmu = __fadd_rn(xmu, a.a.ws_xmu[o]);
+      if (kMode == 2) xmu_d = __fadd_rn(xmu_d, a.d.ws_xmu[o]);
+    }
+  }
+  const int slot = ty * cols + threadIdx.x;
+  for (int off = a.block_y / 2; off > 0; off >>= 1) {
+    if (ty < 2 * off) {
+      s_dy[slot] = dy;
+      s_xmu[slot] = xmu;
+      if (kMode == 2) s_xmu_d[slot] = xmu_d;
+    }
+    __syncthreads();
+    if (ty < off) {
+      const int o = slot + off * cols;
+      dy = __fadd_rn(dy, s_dy[o]);
+      xmu = __fadd_rn(xmu, s_xmu[o]);
+      if (kMode == 2) xmu_d = __fadd_rn(xmu_d, s_xmu_d[o]);
+    }
+    __syncthreads();
+  }
+  if (ty == 0 && live) bwd_finish<kMode>(a, c, dy, xmu, xmu_d);
+}
+
+// dx = bf16(fma(-f1, x - mean, fma(-sum_dy, n, dz)) * f2) per side; the forward's physical scheme
+struct BwdColumn {
+  float mean[kVec], f1[kVec], f2[kVec];
+};
+
+__device__ __forceinline__ void load_elemt_column(const BwdSide& s, float norm, int v, BwdColumn& c) {
+#pragma unroll
+  for (int k = 0; k < kVec; ++k) {
+    const int ch = v * kVec + k;
+    const float inv = s.invstd[ch];
+    c.mean[k] = s.mean[ch];
+    c.f1[k] = __fmul_rn(__fmul_rn(__fmul_rn(inv, inv), s.sum_xmu[ch]), norm);
+    c.f2[k] = __fmul_rn(__bfloat162float(s.weight[ch]), inv);
+  }
+}
+
+__device__ __forceinline__ uint32_t elemt_bits(float t, float x, const BwdColumn& c, int k) {
+  return bf16_bits(__fmul_rn(__fmaf_rn(-c.f1[k], __fsub_rn(x, c.mean[k]), t), c.f2[k]));
+}
+
+template <int kMode>
+__global__ void __launch_bounds__(kBnThreads) bn_bwd_elemt_kernel(const BwdArgs p) {
+  const int v = blockIdx.y * blockDim.x + threadIdx.x;
+  if (v >= p.vecs) return;
+  BwdColumn ea, ed;
+  Column ca;  // mode 0: the forward's parameters, for the mask
+  float sdy[kVec];
+  load_elemt_column(p.a, p.norm, v, ea);
+  if (kMode == 2) load_elemt_column(p.d, p.norm, v, ed);
+  if (kMode == 0) load_bwd_column(p.a, p.bias, v, ca);
+#pragma unroll
+  for (int k = 0; k < kVec; ++k) sdy[k] = p.sum_dy[v * kVec + k];
+  const uint4* g = kMode == 0 ? p.gy : p.dz;
+
+  const int64_t stride = (int64_t)gridDim.x * blockDim.y;
+  const uint4 zero = make_uint4(0, 0, 0, 0);
+  for (int64_t row = (int64_t)blockIdx.x * blockDim.y + threadIdx.y; row < p.rows;
+       row += stride * kRowUnroll) {
+    uint4 qg[kRowUnroll], qx[kRowUnroll], qd[kRowUnroll];
+#pragma unroll
+    for (int u = 0; u < kRowUnroll; ++u) {
+      const int64_t r = row + u * stride;
+      qg[u] = qx[u] = qd[u] = zero;
+      if (r < p.rows) {
+        const int64_t i = r * p.vecs + v;
+        qg[u] = __ldg(g + i);
+        qx[u] = __ldg(p.a.x + i);
+        if (kMode == 2) qd[u] = __ldg(p.d.x + i);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kRowUnroll; ++u) {
+      const int64_t r = row + u * stride;
+      if (r >= p.rows) continue;
+      uint32_t oa[4], od[4];
+#pragma unroll
+      for (int k = 0; k < kVec; ++k) {
+        const int w = k >> 1, h = k & 1;
+        const float x = widen(word(qx[u], w), h);
+        float dz = widen(word(qg[u], w), h);
+        if (kMode == 0) dz = relu_grad(dz, bn_apply(x, ca, k));
+        const float t = __fmaf_rn(-sdy[k], p.norm, dz);
+        const uint32_t ba = elemt_bits(t, x, ea, k);
+        oa[w] = h ? (oa[w] | (ba << 16)) : ba;
+        if (kMode == 2) {
+          const uint32_t bd = elemt_bits(t, widen(word(qd[u], w), h), ed, k);
+          od[w] = h ? (od[w] | (bd << 16)) : bd;
+        }
+      }
+      const int64_t i = r * p.vecs + v;
+      if (p.a.dx) p.a.dx[i] = make_uint4(oa[0], oa[1], oa[2], oa[3]);
+      if (kMode == 2 && p.d.dx) p.d.dx[i] = make_uint4(od[0], od[1], od[2], od[3]);
+    }
+  }
+}
+
 }  // namespace
 
 // ---- host side --------------------------------------------------------------------------------
@@ -385,10 +710,13 @@ struct DevInfo {
 };
 constexpr int kMaxDevices = 64;
 DevInfo g_dev[kMaxDevices];
-std::atomic<int> g_blocks_per_sm[3];
+std::atomic<int> g_blocks_per_sm[6];  // forward modes 0-2, then the backward's elementwise modes
 
-template <int kMode>
-int launch(const BnArgs& a, void* stream) {
+// One thread per 8-channel vector column, walking rows with a grid stride; the grid is sized from
+// the SM count and the kernel's occupancy.  `slot` caches that occupancy.
+template <typename Args>
+int launch_rows(void (*kernel)(Args), int slot, const Args& a, int64_t rows, int vecs,
+                void* stream) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices)
     return fail(TOK_ERR_CUDA, "bn_fused: no current CUDA device");
@@ -398,24 +726,28 @@ int launch(const BnArgs& a, void* stream) {
     if (sms <= 0) sms = 1;
     g_dev[dev].sms.store(sms, std::memory_order_relaxed);
   }
-  int per_sm = g_blocks_per_sm[kMode].load(std::memory_order_relaxed);
+  int per_sm = g_blocks_per_sm[slot].load(std::memory_order_relaxed);
   if (per_sm == 0) {
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bn_fused_fwd_kernel<kMode>,
-                                                  kBnThreads, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kBnThreads, 0);
     if (per_sm <= 0) per_sm = 1;
-    g_blocks_per_sm[kMode].store(per_sm, std::memory_order_relaxed);
+    g_blocks_per_sm[slot].store(per_sm, std::memory_order_relaxed);
   }
-  const int tile = a.vecs < kMaxTileVecs ? a.vecs : kMaxTileVecs;
+  const int tile = vecs < kMaxTileVecs ? vecs : kMaxTileVecs;
   const dim3 block(tile, kBnThreads / tile);
-  const int tiles = (a.vecs + tile - 1) / tile;
-  const int64_t row_blocks = (a.rows + block.y - 1) / block.y;
+  const int tiles = (vecs + tile - 1) / tile;
+  const int64_t row_blocks = (rows + block.y - 1) / block.y;
   int64_t want = (int64_t)sms * per_sm / tiles;
   if (want < 1) want = 1;
   const dim3 grid((unsigned)(row_blocks < want ? row_blocks : want), tiles);
-  bn_fused_fwd_kernel<kMode><<<grid, block, 0, (cudaStream_t)stream>>>(a);
+  kernel<<<grid, block, 0, (cudaStream_t)stream>>>(a);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(TOK_ERR_CUDA, "bn_fused launch: %s", cudaGetErrorString(e));
   return TOK_OK;
+}
+
+template <int kMode>
+int launch(const BnArgs& a, void* stream) {
+  return launch_rows(bn_fused_fwd_kernel<kMode>, kMode, a, a.rows, a.vecs, stream);
 }
 
 bool misaligned(const void* p) { return ((uintptr_t)p & 15u) != 0; }
@@ -458,6 +790,83 @@ int check_stats_shape(const char* who, int64_t rows, int channels) {
   if (channels % kVec != 0)
     return fail(TOK_ERR_ALIGN, "%s: channels %d is not a multiple of %d", who, channels, kVec);
   return TOK_OK;
+}
+
+int check_act(const char* who, const char* what, const void* p, bool required) {
+  if (!p) return required ? fail(TOK_ERR_INVALID, "%s: null %s", who, what) : TOK_OK;
+  if (misaligned(p)) return fail(TOK_ERR_ALIGN, "%s: %s is not 16-byte aligned", who, what);
+  return TOK_OK;
+}
+
+BwdSide bwd_side(const void* x, const float* mean, const float* invstd, const void* weight,
+                 void* dx, void* grad_weight, void* grad_bias) {
+  BwdSide s{};
+  s.x = (const uint4*)x;
+  s.mean = mean;
+  s.invstd = invstd;
+  s.weight = (const __nv_bfloat16*)weight;
+  s.grad_weight = (__nv_bfloat16*)grad_weight;
+  s.grad_bias = (__nv_bfloat16*)grad_bias;
+  s.dx = (uint4*)dx;
+  return s;
+}
+
+// Checks what every mode shares, lays the workspace out and runs the reduction, its finish and
+// (when a dx is asked for) the elementwise pass.
+template <int kMode>
+int bn_bwd(const char* who, BwdArgs& a, int64_t rows, int channels, void* workspace,
+           void* cuda_stream) {
+  int rc = check_stats_shape(who, rows, channels);
+  if (rc == TOK_OK) rc = check_act(who, "gy", a.gy, true);
+  if (rc == TOK_OK) rc = check_act(who, "x", a.a.x, true);
+  if (rc == TOK_OK) rc = check_act(who, "dx", a.a.dx, false);
+  if (rc == TOK_OK && kMode != 0) rc = check_act(who, "y", a.y, true);
+  if (rc == TOK_OK && kMode != 0) rc = check_act(who, "dz", a.dz, true);
+  if (rc == TOK_OK && kMode == 2) rc = check_act(who, "xd", a.d.x, true);
+  if (rc == TOK_OK && kMode == 2) rc = check_act(who, "dxd", a.d.dx, false);
+  if (rc == TOK_OK) rc = check_act(who, "workspace", workspace, true);
+  if (rc != TOK_OK) return rc;
+  if (!a.a.mean || !a.a.invstd || !a.a.weight || (kMode == 0 && !a.bias) ||
+      (kMode == 2 && (!a.d.mean || !a.d.invstd || !a.d.weight)))
+    return fail(TOK_ERR_INVALID, "%s: null pointer argument", who);
+  if (!device_ready()) return fail(TOK_ERR_NO_DEVICE, "%s needs a CUDA GPU (no CPU fallback)", who);
+
+  const BnStatsGeom g = bn_stats_geometry((int)rows, channels);
+  const int sums = kMode == 2 ? 3 : 2;
+  float* f = (float*)workspace;
+  a.sum_dy = f;
+  a.a.sum_xmu = f + channels;
+  if (kMode == 2) a.d.sum_xmu = f + 2 * channels;
+  if (g.grid_y > 1) {
+    float* part = f + (int64_t)sums * channels;
+    const int64_t n = (int64_t)g.grid_y * channels;
+    a.ws_dy = part;
+    a.a.ws_xmu = part + n;
+    if (kMode == 2) a.d.ws_xmu = part + 2 * n;
+  }
+  a.rows = (int)rows;
+  a.channels = channels;
+  a.vecs = channels / kVec;
+  a.block_y = g.block_y;
+  a.grid_y = g.grid_y;
+  a.loop_count = g.loop_count;
+  a.norm = (float)(1.0 / (double)rows);  // ATen: norm_fct = 1.0 / reduction_size, passed as float
+
+  int tile = kBwdPartialThreads / (kStatsChains * g.block_y);
+  if (tile > a.vecs) tile = a.vecs;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  bn_bwd_partial_kernel<kMode><<<dim3((a.vecs + tile - 1) / tile, g.grid_y),
+                                 dim3(kStatsChains * tile, g.block_y), 0, st>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(TOK_ERR_CUDA, "bn_bwd_partial launch: %s", cudaGetErrorString(e));
+  if (g.grid_y > 1) {
+    const int cols = kStatsThreads / g.block_y;
+    bn_bwd_finish_kernel<kMode><<<(channels + cols - 1) / cols, dim3(cols, g.block_y), 0, st>>>(a);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(TOK_ERR_CUDA, "bn_bwd_finish launch: %s", cudaGetErrorString(e));
+  }
+  if (!a.a.dx && !(kMode == 2 && a.d.dx)) return TOK_OK;
+  return launch_rows(bn_bwd_elemt_kernel<kMode>, 3 + kMode, a, rows, a.vecs, cuda_stream);
 }
 
 }  // namespace
@@ -581,4 +990,51 @@ extern "C" int tok_bn_stats_fwd(const void* x, int64_t rows, int channels, doubl
       return fail(TOK_ERR_CUDA, "bn_stats_finish launch: %s", cudaGetErrorString(e));
   }
   return TOK_OK;
+}
+
+extern "C" int64_t tok_bn_bwd_workspace_bytes(int64_t rows, int channels, int mode) {
+  const char* who = "tok_bn_bwd_workspace_bytes";
+  const int rc = check_stats_shape(who, rows, channels);
+  if (rc != TOK_OK) return rc;
+  if (mode < 0 || mode > 2) return fail(TOK_ERR_INVALID, "%s: mode %d is not 0, 1 or 2", who, mode);
+  return bn_bwd_workspace(bn_stats_geometry((int)rows, channels), channels, mode == 2 ? 3 : 2);
+}
+
+extern "C" int tok_bn_relu_bwd(const void* gy, const void* x, const float* mean,
+                               const float* invstd, const void* weight, const void* bias, void* dx,
+                               void* grad_weight, void* grad_bias, int64_t rows, int channels,
+                               void* workspace, void* cuda_stream) {
+  BwdArgs a{};
+  a.a = bwd_side(x, mean, invstd, weight, dx, grad_weight, grad_bias);
+  a.gy = (const uint4*)gy;
+  a.bias = (const __nv_bfloat16*)bias;
+  return bn_bwd<0>("tok_bn_relu_bwd", a, rows, channels, workspace, cuda_stream);
+}
+
+extern "C" int tok_bn_add_relu_bwd(const void* gy, const void* y, const void* x, const float* mean,
+                                   const float* invstd, const void* weight, void* dz, void* dx,
+                                   void* grad_weight, void* grad_bias, int64_t rows, int channels,
+                                   void* workspace, void* cuda_stream) {
+  BwdArgs a{};
+  a.a = bwd_side(x, mean, invstd, weight, dx, grad_weight, grad_bias);
+  a.gy = (const uint4*)gy;
+  a.y = (const uint4*)y;
+  a.dz = (uint4*)dz;
+  return bn_bwd<1>("tok_bn_add_relu_bwd", a, rows, channels, workspace, cuda_stream);
+}
+
+extern "C" int tok_bn2_add_relu_bwd(const void* gy, const void* y, const void* x, const float* mean,
+                                    const float* invstd, const void* weight, const void* xd,
+                                    const float* mean_d, const float* invstd_d,
+                                    const void* weight_d, void* dz, void* dx, void* grad_weight,
+                                    void* grad_bias, void* dxd, void* grad_weight_d,
+                                    void* grad_bias_d, int64_t rows, int channels, void* workspace,
+                                    void* cuda_stream) {
+  BwdArgs a{};
+  a.a = bwd_side(x, mean, invstd, weight, dx, grad_weight, grad_bias);
+  a.d = bwd_side(xd, mean_d, invstd_d, weight_d, dxd, grad_weight_d, grad_bias_d);
+  a.gy = (const uint4*)gy;
+  a.y = (const uint4*)y;
+  a.dz = (uint4*)dz;
+  return bn_bwd<2>("tok_bn2_add_relu_bwd", a, rows, channels, workspace, cuda_stream);
 }

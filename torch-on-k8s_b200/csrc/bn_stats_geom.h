@@ -59,4 +59,13 @@ inline int64_t bn_stats_workspace(const BnStatsGeom& g, int channels) {
   return counts + 2 * (int64_t)g.grid_y * channels * 4;
 }
 
+// The backward reduction (ATen's batch_norm_backward_reduce_channels_last_kernel) is launched with the
+// same flexible_launch_configs(coop = true), so it has this geometry too.  Its workspace: `sums`
+// float[channels] results (sum_dy, then one sum_dy_xmu per batch norm), then, when grid_y > 1, the
+// per logical block partials float[sums][grid_y][channels].
+inline int64_t bn_bwd_workspace(const BnStatsGeom& g, int channels, int sums) {
+  const int64_t results = (int64_t)sums * channels * 4;
+  return g.grid_y == 1 ? results : results * (1 + g.grid_y);
+}
+
 }  // namespace tok

@@ -14,10 +14,17 @@ from libtok8s's statistics kernels, which perform the arithmetic of ATen's chann
 kernel and of `torch.batch_norm_update_stats` in the same order, bit for bit, with 16-byte loads
 and more loads in flight; one libtok8s kernel then applies the normalisation with ATen's exact
 float expression, adds the residual (or the second, downsample batch norm) and applies the ReLU,
-writing one bf16 tensor where the stock composition writes and re-reads two or three.  The backward is the stock
-one: `threshold_backward` on the saved output, then `native_batch_norm_backward` with the saved
-mean and invstd, saving the same activations stock autograd saves (the batch-norm inputs and the
-ReLU output).
+writing one bf16 tensor where the stock composition writes and re-reads two or three.
+
+The backward folds `threshold_backward` into libtok8s's batch-norm backward kernels, which perform
+the arithmetic of ATen's channels_last backward reduce and elementwise kernels in the same order, bit
+for bit: one reduction pass, then one elementwise pass (skipped when x needs no gradient).  bn_relu
+saves x, mean, invstd and var instead of its output (and keeps weight and bias, checking their
+versions), and recomputes the ReLU mask from x; the other two save their output, whose mask also
+gives the residual's gradient.  No activation is saved that the stock composition does not save.  A gy the kernels cannot read (not bf16
+channels_last-contiguous and 16-byte aligned like x, e.g. the zero-stride gy of `y.sum()`) takes
+the stock backward: `threshold_backward` on the output (recomputed for bn_relu), then
+`native_batch_norm_backward` with the saved mean and invstd.
 
 The fused path is taken when the inputs allow it: CUDA, bf16 activations and batch-norm tensors,
 channels_last-contiguous 4-D activations with C % 8 == 0 and 16-byte aligned data, a module in
@@ -117,10 +124,15 @@ class _BnAddRelu(torch.autograd.Function):
                                               ch, stream)
         _ffi.check(rc)
         ctx.bn, ctx.bnd, ctx.mode = bn, bnd, mode
-        if mode == 2:
-            ctx.save_for_backward(x, mean, invstd, other, mean_d, invstd_d, y)
+        if mode == 0:
+            # y is recomputed from x where it is needed; var only for the stock backward's y.
+            # weight and bias are kept with their versions, which backward checks as autograd would.
+            ctx.save_for_backward(x, mean, invstd, var)
+            ctx.params = (weight, bias, weight._version, bias._version)
+        elif mode == 1:
+            ctx.save_for_backward(x, mean, invstd, y, weight)
         else:
-            ctx.save_for_backward(x, mean, invstd, y)
+            ctx.save_for_backward(x, mean, invstd, other, mean_d, invstd_d, y, weight, weight_d)
         return y
 
     @staticmethod
@@ -128,21 +140,90 @@ class _BnAddRelu(torch.autograd.Function):
     def backward(ctx, gy):
         need = ctx.needs_input_grad
         saved = ctx.saved_tensors
-        y = saved[-1]
+        x = saved[0]
+        if ctx.mode == 0:
+            weight, bias, vw, vb = ctx.params
+            if weight._version != vw or bias._version != vb:
+                raise RuntimeError("bn_relu: the batch norm's weight or bias was modified by an "
+                                   "inplace operation after the forward")
+        if _same(x, gy):
+            return _fused_backward(ctx, gy, need, saved)
+        if ctx.mode == 0:
+            x, mean, invstd, var = saved
+            y = torch.empty_like(x)
+            with torch.cuda.device(x.device):
+                stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
+                rc = _ffi.lib().tok_bn_relu_fwd(_ptr(x), _ptr(mean), _ptr(var), _ptr(weight),
+                                                _ptr(bias), ctx.bn.eps, _ptr(torch.empty_like(mean)),
+                                                _ptr(y), x.numel() // x.shape[1], x.shape[1], stream)
+            _ffi.check(rc)
+        elif ctx.mode == 1:
+            x, mean, invstd, y, _ = saved
+        else:
+            x, mean, invstd, xd, mean_d, invstd_d, y, _, _ = saved
         g = torch.ops.aten.threshold_backward(gy, y, 0)
         dxd = dwd = dbd = dr = None
         if ctx.mode == 2:
-            x, mean, invstd, xd, mean_d, invstd_d, _ = saved
             # the downsample branch first, as the unfused graph orders it
             dxd, dwd, dbd = _bn_backward(g, xd, ctx.bnd, mean_d, invstd_d, [need[3], need[4], need[5]])
-        else:
-            x, mean, invstd, _ = saved
-            if ctx.mode == 1 and need[3]:
-                dr = g
+        elif ctx.mode == 1 and need[3]:
+            dr = g
         dx, dw, db = _bn_backward(g, x, ctx.bn, mean, invstd, [need[0], need[1], need[2]])
         if ctx.mode == 2:
             return dx, dw, db, dxd, dwd, dbd, None, None, None
         return dx, dw, db, dr, None, None, None, None, None
+
+
+def _fused_backward(ctx, gy, need, saved):
+    """threshold_backward + native_batch_norm_backward through libtok8s, for a gy laid out as x."""
+    mode = ctx.mode
+    x = saved[0]
+    rows, ch = x.numel() // x.shape[1], x.shape[1]
+    lib = _ffi.lib()
+    nbytes = lib.tok_bn_bwd_workspace_bytes(rows, ch, mode)
+    if nbytes < 0:
+        _ffi.check(nbytes)
+    work = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+
+    def out(i, like):
+        return torch.empty_like(like) if need[i] else None
+
+    def ptr(t):
+        return None if t is None else _ptr(t)
+
+    dx = out(0, x)
+    with torch.cuda.device(x.device):
+        stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
+        if mode == 0:
+            _, mean, invstd, _ = saved
+            weight, bias = ctx.params[:2]
+            dw, db = out(1, weight), out(2, weight)
+            rc = lib.tok_bn_relu_bwd(_ptr(gy), _ptr(x), _ptr(mean), _ptr(invstd), _ptr(weight),
+                                     _ptr(bias), ptr(dx), ptr(dw), ptr(db), rows, ch, _ptr(work),
+                                     stream)
+            grads = (dx, dw, db, None)
+        elif mode == 1:
+            _, mean, invstd, y, weight = saved
+            dw, db = out(1, weight), out(2, weight)
+            dz = torch.empty_like(x)
+            rc = lib.tok_bn_add_relu_bwd(_ptr(gy), _ptr(y), _ptr(x), _ptr(mean), _ptr(invstd),
+                                         _ptr(weight), _ptr(dz), ptr(dx), ptr(dw), ptr(db), rows, ch,
+                                         _ptr(work), stream)
+            grads = (dx, dw, db, dz if need[3] else None)
+        else:
+            _, mean, invstd, xd, mean_d, invstd_d, y, weight, weight_d = saved
+            dw, db = out(1, weight), out(2, weight)
+            dxd = out(3, xd)
+            dwd, dbd = out(4, weight_d), out(5, weight_d)
+            dz = torch.empty_like(x)
+            rc = lib.tok_bn2_add_relu_bwd(_ptr(gy), _ptr(y), _ptr(x), _ptr(mean), _ptr(invstd),
+                                          _ptr(weight), _ptr(xd), _ptr(mean_d), _ptr(invstd_d),
+                                          _ptr(weight_d), _ptr(dz), ptr(dx), ptr(dw), ptr(db),
+                                          ptr(dxd), ptr(dwd), ptr(dbd), rows, ch, _ptr(work), stream)
+            _ffi.check(rc)
+            return dx, dw, db, dxd, dwd, dbd, None, None, None
+    _ffi.check(rc)
+    return grads + (None,) * 5
 
 
 def bn_relu(x: torch.Tensor, bn: torch.nn.Module) -> torch.Tensor:
