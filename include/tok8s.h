@@ -301,6 +301,42 @@ int tok_adam_master_step(const tok_adam_segment_t* segments, int count, int64_t 
                          double lr, double beta1, double beta2, double eps, double weight_decay,
                          int decoupled, int amsgrad, double step, void* cuda_stream);
 
+/* tok_sgd_master_step / tok_adam_master_step with gradient clipping: the same step, table and rules,
+ * with grad = f32(segment.grad) * *grad_coef (one rounding) as the master's gradient, the first
+ * operation on it, before weight decay — the bits of torch.nn.utils.clip_grad_norm_ having multiplied
+ * master.grad by its clamped coefficient (_foreach_mul_) before the optimizer step.  `grad_coef` is a
+ * DEVICE fp32 scalar, read by the kernel, so it may be formed on `cuda_stream` just before.  Returns
+ * what the unclipped entry point returns, and TOK_ERR_INVALID for a null `grad_coef`. */
+int tok_sgd_master_step_clipped(const tok_sgd_segment_t* segments, int count, int64_t chunks,
+                                int dtype, double lr, double momentum, double dampening,
+                                double weight_decay, int nesterov, int fresh,
+                                const float* grad_coef, void* cuda_stream);
+int tok_adam_master_step_clipped(const tok_adam_segment_t* segments, int count, int64_t chunks,
+                                 int dtype, double lr, double beta1, double beta2, double eps,
+                                 double weight_decay, int decoupled, int amsgrad, double step,
+                                 const float* grad_coef, void* cuda_stream);
+
+/* Per-tensor L2 norms of bf16 / f16 gradients (gradient clipping in torch_on_k8s_b200/optim.py): for
+ * every segment, norms[slot] receives the bits of torch._foreach_norm([f32(grad)], 2)[0] — ATen's
+ * chunking, per-thread accumulators, FMA squares, block reduction trees and correctly rounded sqrt,
+ * with the accumulator mapping of a fresh fp32 copy of the gradient, wherever the gradient sits.
+ * `segments` is a DEVICE array of `count` entries; entry k's `chunk0` must be the sum of
+ * ceil(numel / TOK_NORM_CHUNK) over the entries before it and `chunks` that sum over all entries.
+ * `partials` is DEVICE fp32 scratch of `chunks` elements (may be NULL when `chunks` is 0); `norms` a
+ * DEVICE fp32 array holding every `slot`.  Two launches.  Returns TOK_ERR_INVALID for a null table or
+ * norms, an empty table, a negative or too large `chunks`, null partials with chunks, a dtype other
+ * than TOK_BF16 / TOK_F16, TOK_ERR_NO_DEVICE without a GPU.  Enqueued on `cuda_stream`, no
+ * synchronisation. */
+#define TOK_NORM_CHUNK 65536
+typedef struct tok_norm_segment {
+  const void* grad; /* bf16 / f16[numel], the parameter's gradient (anywhere in its bucket)       */
+  int64_t numel;
+  int64_t chunk0;   /* index of this segment's first chunk, and of its first partial              */
+  int64_t slot;     /* index of its norm in `norms`                                               */
+} tok_norm_segment_t;
+int tok_grad_norms(const tok_norm_segment_t* segments, int count, int64_t chunks, int dtype,
+                   float* partials, float* norms, void* cuda_stream);
+
 /* Which algorithm AUTO picks for `wire_bytes` on this communicator. */
 int tok_allreduce_algo(tok_comm_t* comm, size_t wire_bytes, int* algo);
 /* Number of kernels this communicator has launched so far (bench.py's gpu_launches): exchange,

@@ -26,7 +26,9 @@ class BucketAllreduceHook:
 
     optimizer (a MasterWeightSGD, MasterWeightAdam or MasterWeightAdamW): each bucket's optimizer
     step is enqueued on the same stream right behind its exchange, before the Future is set;
-    optimizer.step() then only orders the current stream after that stream.
+    optimizer.step() then only orders the current stream after that stream.  An optimizer with
+    max_grad_norm enqueues only the bucket's gradient norms there; its step() forms the global norm
+    and steps every bucket.
     """
 
     def __init__(self, comm: Communicator, *, wire_dtype: Optional[torch.dtype] = None,

@@ -92,7 +92,8 @@ class ElasticDataParallel(torch.nn.Module):
         """Average the gradient buckets across the current peer group (in place, zero-copy).
         optimizer (a MasterWeightSGD, MasterWeightAdam or MasterWeightAdamW): each bucket's step is
         enqueued right behind its exchange; optimizer.step() then launches nothing for these
-        parameters."""
+        parameters.  With max_grad_norm only the bucket's gradient norms are enqueued there, and
+        optimizer.step() steps every bucket once the global norm exists."""
         world = self.comm.world
         for k, b in enumerate(self.buckets):   # PRE scale: the same function as built-in DDP
             self.comm.allreduce_bucket(b, b, scale=1.0 / world, algo=self.algo, stream=stream)

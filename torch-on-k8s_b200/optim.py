@@ -22,10 +22,27 @@ then only orders the current stream after those streams (and steps whatever no b
 That is the contract of torch's ddp_comm_hooks.optimizer_overlap_hooks: a bucket is ready only after
 every autograd node that reads its parameters has run, so its parameters may change while the rest of
 backward runs.
+
+Gradient clipping.  With an overlapped optimizer the parameters and masters have already been
+updated when `loss.backward()` returns, so `torch.nn.utils.clip_grad_norm_(model.parameters(), c)`
+after backward scales bf16 gradients nothing reads again: the update was not clipped.  Pass
+`max_grad_norm=c` instead.  One step then gives the bits of
+
+    for each master: master.grad = p.grad.float()      (None where p.grad is None)
+    total = torch.nn.utils.clip_grad_norm_(masters, c)  # norm_type 2, foreach
+    opt.step()                                           # stock foreach SGD / Adam / AdamW
+    p.copy_(master)
+
+and `opt.grad_norm` holds `total` (the pre-clip norm, a 0-d fp32 CUDA tensor).  A global norm needs
+every gradient, so each bucket's hook only enqueues its per-tensor norms (csrc/grad_norm.cu) behind
+its exchange; step() forms the total and the coefficient with clip_grad_norm_'s own torch
+expressions on the device and launches every bucket's clipped step then.  Clipping thus moves the
+steps from behind each exchange to after backward.  Norm types other than 2 are not supported.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Dict, Iterable, List, Optional, Tuple
 
 import torch
@@ -33,6 +50,7 @@ import torch
 from . import _ffi
 
 CHUNK = 4096   # TOK_SGD_CHUNK
+NORM_CHUNK = 65536   # TOK_NORM_CHUNK: ATen's _foreach_norm chunk
 _DTYPES = {torch.bfloat16: _ffi.TOK_BF16, torch.float16: _ffi.TOK_F16}
 
 
@@ -59,6 +77,27 @@ def segment_table(entries) -> Tuple[List[tuple], int]:
     return rows, chunks
 
 
+def norm_table(entries) -> Tuple[List[tuple], int]:
+    """Rows of tok_norm_segment_t — (grad, numel, chunk0, slot) as integers — for [(grad, slot)],
+    and the total number of chunks."""
+    rows, chunks = [], 0
+    for g, slot in entries:
+        n = g.numel()
+        rows.append((g.data_ptr(), n, chunks, slot))
+        chunks += -(-n // NORM_CHUNK)
+    return rows, chunks
+
+
+def _check_max_grad_norm(max_grad_norm) -> Optional[float]:
+    if max_grad_norm is None:
+        return None
+    if isinstance(max_grad_norm, bool) or not isinstance(max_grad_norm, (int, float)) or \
+            not math.isfinite(max_grad_norm) or max_grad_norm <= 0:
+        raise ValueError("max_grad_norm must be a finite number > 0 or None, got %r"
+                         % (max_grad_norm,))
+    return float(max_grad_norm)
+
+
 class _MasterWeightOptimizer(torch.optim.Optimizer):
     """What the master-weight optimizers share: the parameter checks, fp32 masters, the fp32 restore
     of state_dict, bucket and whole-group stepping with the stream ordering, and the device tables
@@ -68,11 +107,19 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
     _FP32_STATE: Tuple[str, ...] = ("master_param",)   # state restored to fp32 by load_state_dict
     _FP32_HINT = ""                                      # the stock optimizer for fp32 parameters
 
-    def __init__(self, params, defaults: dict):
+    def __init__(self, params, defaults: dict, max_grad_norm: Optional[float] = None,
+                 error_if_nonfinite: bool = False):
         self._group_of: Dict[int, int] = {}          # id(param) -> index of its param group
+        self._slot_of: Dict[int, int] = {}           # id(param) -> position in param-group order
         self._tables: Dict[tuple, tuple] = {}        # launch key -> (rows, device table)
-        self._stepped: set = set()                   # id(param) stepped behind an exchange
-        self._streams: List[torch.cuda.Stream] = []  # streams those steps ran on
+        self._stepped: set = set()                   # id(param) stepped (or normed) by a bucket
+        self._streams: List[torch.cuda.Stream] = []  # streams those launches ran on
+        self._pending: List[tuple] = []              # clipping: (index, {group: pairs}) per bucket
+        self._norms: Optional[torch.Tensor] = None   # clipping: fp32 norm per slot, on the device
+        self._present: Optional[tuple] = None        # clipping: (slots, device index) of the last gather
+        self.max_grad_norm = _check_max_grad_norm(max_grad_norm)
+        self.error_if_nonfinite = bool(error_if_nonfinite)
+        self.grad_norm: Optional[torch.Tensor] = None   # clipping: the last step's pre-clip norm
         self.table_uploads = 0
         super().__init__(params, defaults)
 
@@ -88,6 +135,7 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                                     self._FP32_HINT))
         for p in group["params"]:
             self._group_of[id(p)] = len(self.param_groups) - 1
+            self._slot_of[id(p)] = len(self._slot_of)
             self.state[p]["master_param"] = p.detach().to(torch.float32, copy=True,
                                                           memory_format=torch.preserve_format)
 
@@ -108,13 +156,19 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         raise NotImplementedError
 
     def _kernel(self, group: dict, table: torch.Tensor, count: int, chunks: int, dtype: int, arg,
-                stream: torch.cuda.Stream) -> None:
+                stream: torch.cuda.Stream, coef: Optional[torch.Tensor]) -> None:
+        """One launch; with `coef` (the device clip coefficient) the clipped kernel."""
         raise NotImplementedError
 
-    def _launch(self, group: dict, pairs, key: tuple,
-                stream: Optional[torch.cuda.Stream] = None) -> None:
-        """Step [(param, grad)] of one param group with the launches _split gives, on `stream` (which
-        must then be current) or the current stream."""
+    def _table(self, key: tuple, rows: List[tuple], dev: torch.device) -> torch.Tensor:
+        cached = self._tables.get(key)
+        if cached is None or cached[0] != rows:
+            # uploaded on the launching stream, the only stream that reads it
+            cached = self._tables[key] = (rows, torch.tensor(rows, dtype=torch.int64).to(dev))
+            self.table_uploads += 1
+        return cached[1]
+
+    def _check_pairs(self, pairs) -> None:
         name = type(self).__name__
         for p, g in pairs:
             if g.is_sparse:
@@ -127,28 +181,108 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             if not p.is_cuda:
                 raise RuntimeError("%s steps CUDA parameters only: the kernel has no CPU fallback"
                                    % name)
+
+    def _launch(self, group: dict, pairs, key: tuple, stream: Optional[torch.cuda.Stream] = None,
+                coef: Optional[torch.Tensor] = None) -> None:
+        """Step [(param, grad)] of one param group with the launches _split gives, on `stream` (which
+        must then be current) or the current stream; with `coef`, clipped."""
+        self._check_pairs(pairs)
         stream = stream or torch.cuda.current_stream(pairs[0][0].device)
         for sub, entries, arg in self._split(group, pairs):
             if not entries:
                 continue
             dev = entries[0][1].device
             rows, chunks = segment_table(entries)
-            k = key + (sub,)
-            cached = self._tables.get(k)
-            if cached is None or cached[0] != rows:
-                # uploaded on `stream`, the only stream that reads it
-                cached = self._tables[k] = (rows, torch.tensor(rows, dtype=torch.int64).to(dev))
-                self.table_uploads += 1
+            table = self._table(key + (sub,), rows, dev)
             with torch.cuda.device(dev):
-                self._kernel(group, cached[1], len(rows), chunks, _DTYPES[entries[0][1].dtype], arg,
-                             stream)
+                self._kernel(group, table, len(rows), chunks, _DTYPES[entries[0][1].dtype], arg,
+                             stream, coef)
+
+    # ---- clipping --------------------------------------------------------------------------------
+    def _norm_buffer(self, dev: torch.device) -> torch.Tensor:
+        """One fp32 norm per parameter slot, kept across steps (allocated on the current stream)."""
+        if self._norms is None or self._norms.device != dev or \
+                self._norms.numel() != len(self._slot_of):
+            self._norms = torch.zeros(len(self._slot_of), dtype=torch.float32, device=dev)
+            self._present = None
+        return self._norms
+
+    def _launch_norms(self, pairs, key: tuple, norms: torch.Tensor,
+                      stream: torch.cuda.Stream) -> None:
+        """Enqueue on `stream` (current) the norms of [(param, grad)] into their slots of `norms`: one
+        tok_grad_norms call (two kernels) per gradient dtype."""
+        by_dtype: Dict[torch.dtype, list] = {}
+        for p, g in pairs:
+            if g.device != norms.device:
+                raise ValueError("%s clips gradients on one device; got %s and %s"
+                                 % (type(self).__name__, g.device, norms.device))
+            by_dtype.setdefault(g.dtype, []).append((g, self._slot_of[id(p)]))
+        for dtype, entries in by_dtype.items():
+            rows, chunks = norm_table(entries)
+            table = self._table(key + (str(dtype),), rows, norms.device)
+            # caching-allocator scratch on `stream`: freed back to it after this call
+            partials = torch.empty(chunks, dtype=torch.float32, device=norms.device)
+            with torch.cuda.device(norms.device):
+                _ffi.check(_ffi.lib().tok_grad_norms(
+                    C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype],
+                    C.c_void_p(partials.data_ptr() if chunks else 0),
+                    C.c_void_p(norms.data_ptr()), C.c_void_p(stream.cuda_stream)))
+
+    def _clip_step(self) -> None:
+        """step() with max_grad_norm: the norms no bucket covered, clip_grad_norm_'s total and
+        coefficient, then every clipped launch — on the current stream, after the bucket streams."""
+        pending, self._pending = self._pending, []
+        rest = []
+        for gi, group in enumerate(self.param_groups):
+            pairs = [(p, p.grad) for p in group["params"]
+                     if p.grad is not None and id(p) not in self._stepped]
+            if pairs:
+                rest.append((gi, pairs))
+        present = tuple(self._slot_of[id(p)] for group in self.param_groups for p in group["params"]
+                        if id(p) in self._stepped or p.grad is not None)
+        self._stepped.clear()
+        self._streams.clear()
+        if not present:
+            self.grad_norm = torch.tensor(0.0)   # what clip_grad_norm_ returns without gradients
+            return
+        pairs = [pg for _, prs in rest for pg in prs]
+        self._check_pairs(pairs)
+        dev = (pairs[0][0] if pairs else next(iter(pending[0][1].values()))[0][0]).device
+        stream = torch.cuda.current_stream(dev)
+        norms = self._norm_buffer(dev)
+        if pairs:
+            self._launch_norms(pairs, ("norm", "group"), norms, stream)
+        if len(present) != norms.numel():
+            # clip_grad_norm_ stacks only the gradients that exist: gather their slots, in order
+            if self._present is None or self._present[0] != present:
+                self._present = (present, torch.tensor(present, dtype=torch.int64).to(dev))
+            norms = norms.index_select(0, self._present[1])
+        # torch.nn.utils.clip_grad_norm_'s own expressions (_get_total_norm, _clip_grads_with_norm_)
+        total = torch.linalg.vector_norm(norms, 2.0)
+        if self.error_if_nonfinite and torch.logical_or(total.isnan(), total.isinf()):
+            raise RuntimeError(
+                f"The total norm of order {2.0} for gradients from "
+                "`parameters` is non-finite, so it cannot be clipped. To disable "
+                "this error and scale the gradients by the non-finite norm anyway, "
+                "set `error_if_nonfinite=False`")
+        coef = torch.clamp(self.max_grad_norm / (total + 1e-6), max=1.0)
+        self.grad_norm = total
+        for index, by_group in pending:
+            for gi, prs in by_group.items():
+                self._launch(self.param_groups[gi], prs, ("clip bucket", index, gi), stream, coef)
+        for gi, prs in rest:
+            self._launch(self.param_groups[gi], prs, ("clip group", gi), stream, coef)
 
     @torch.no_grad()
     def step_bucket(self, params: Iterable[torch.Tensor], grads: Iterable[torch.Tensor], index: int,
                     stream: Optional[torch.cuda.Stream] = None) -> None:
         """Step the parameters of gradient bucket `index` (those this optimizer holds) on `stream`
         (default: the current one), behind whatever that stream already carries — the bucket's
-        exchange.  The next step() orders the current stream after `stream`."""
+        exchange.  The next step() orders the current stream after `stream`.
+
+        With max_grad_norm, enqueue only the bucket's per-tensor gradient norms there and keep the
+        bucket for step(), which steps it once the global norm exists.  `grads` must then hold the
+        averaged gradients until step()."""
         by_group: Dict[int, list] = {}
         for p, g in zip(params, grads):
             gi = self._group_of.get(id(p))
@@ -158,6 +292,17 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             return
         dev = next(iter(by_group.values()))[0][0].device
         stream = stream or torch.cuda.current_stream(dev)
+        if self.max_grad_norm is not None:
+            pairs = [pg for prs in by_group.values() for pg in prs]
+            self._check_pairs(pairs)
+            norms = self._norm_buffer(dev)
+            with torch.cuda.stream(stream):
+                self._launch_norms(pairs, ("norm", "bucket", index), norms, stream)
+            self._pending.append((index, by_group))
+            self._stepped.update(id(p) for p, _ in pairs)
+            if stream not in self._streams:
+                self._streams.append(stream)
+            return
         with torch.cuda.stream(stream):
             for gi, pairs in by_group.items():
                 self._launch(self.param_groups[gi], pairs, ("bucket", index, gi), stream)
@@ -173,6 +318,9 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                 loss = closure()
         for s in self._streams:
             torch.cuda.current_stream(s.device).wait_stream(s)
+        if self.max_grad_norm is not None:
+            self._clip_step()
+            return loss
         for gi, group in enumerate(self.param_groups):
             pairs = [(p, p.grad) for p in group["params"]
                      if p.grad is not None and id(p) not in self._stepped]
@@ -189,7 +337,8 @@ class MasterWeightSGD(_MasterWeightOptimizer):
 
     def __init__(self, params, lr: float, momentum: float = 0.0, dampening: float = 0.0,
                  weight_decay: float = 0.0, nesterov: bool = False, *, maximize: bool = False,
-                 differentiable: bool = False):
+                 differentiable: bool = False, max_grad_norm: Optional[float] = None,
+                 error_if_nonfinite: bool = False):
         if lr < 0.0:
             raise ValueError("Invalid learning rate: %r" % lr)
         if momentum < 0.0:
@@ -201,7 +350,8 @@ class MasterWeightSGD(_MasterWeightOptimizer):
         if maximize or differentiable:
             raise ValueError("MasterWeightSGD supports neither maximize nor differentiable")
         super().__init__(params, dict(lr=lr, momentum=momentum, dampening=dampening,
-                                      weight_decay=weight_decay, nesterov=nesterov))
+                                      weight_decay=weight_decay, nesterov=nesterov),
+                         max_grad_norm, error_if_nonfinite)
 
     def _split(self, group: dict, pairs) -> List[tuple]:
         """One launch per momentum state: fresh buffers (subkey 1), then the rest (subkey 0)."""
@@ -218,11 +368,14 @@ class MasterWeightSGD(_MasterWeightOptimizer):
             old.append((g, p, st["master_param"], m))
         return [(1, fresh, 1), (0, old, 0)]
 
-    def _kernel(self, group, table, count, chunks, dtype, fresh, stream) -> None:
-        _ffi.check(_ffi.lib().tok_sgd_master_step(
-            C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], group["momentum"],
-            group["dampening"], group["weight_decay"], int(group["nesterov"]), fresh,
-            C.c_void_p(stream.cuda_stream)))
+    def _kernel(self, group, table, count, chunks, dtype, fresh, stream, coef) -> None:
+        args = [C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], group["momentum"],
+                group["dampening"], group["weight_decay"], int(group["nesterov"]), fresh]
+        if coef is None:
+            _ffi.check(_ffi.lib().tok_sgd_master_step(*args, C.c_void_p(stream.cuda_stream)))
+        else:
+            _ffi.check(_ffi.lib().tok_sgd_master_step_clipped(
+                *args, C.c_void_p(coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
 
 
 class MasterWeightAdam(_MasterWeightOptimizer):
@@ -235,7 +388,8 @@ class MasterWeightAdam(_MasterWeightOptimizer):
                  eps: float = 1e-8, weight_decay: float = 0.0, amsgrad: bool = False, *,
                  foreach: Optional[bool] = None, maximize: bool = False, capturable: bool = False,
                  differentiable: bool = False, fused: Optional[bool] = None,
-                 decoupled_weight_decay: bool = False):
+                 decoupled_weight_decay: bool = False, max_grad_norm: Optional[float] = None,
+                 error_if_nonfinite: bool = False):
         name = type(self).__name__
         if isinstance(lr, torch.Tensor) or any(isinstance(b, torch.Tensor) for b in betas):
             raise ValueError("%s takes lr and betas as Python floats, not Tensors" % name)
@@ -255,7 +409,8 @@ class MasterWeightAdam(_MasterWeightOptimizer):
             raise ValueError(f"Invalid weight_decay value: {weight_decay}")
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay,
                                       amsgrad=amsgrad,
-                                      decoupled_weight_decay=decoupled_weight_decay))
+                                      decoupled_weight_decay=decoupled_weight_decay),
+                         max_grad_norm, error_if_nonfinite)
 
     def load_state_dict(self, state_dict: dict) -> None:
         super().load_state_dict(state_dict)
@@ -287,12 +442,16 @@ class MasterWeightAdam(_MasterWeightOptimizer):
         ordered = sorted(launches.items(), key=lambda kv: (-kv[0][0], str(kv[0][1])))
         return [(i, entries, step) for i, ((step, _), entries) in enumerate(ordered)]
 
-    def _kernel(self, group, table, count, chunks, dtype, step, stream) -> None:
+    def _kernel(self, group, table, count, chunks, dtype, step, stream, coef) -> None:
         beta1, beta2 = group["betas"]
-        _ffi.check(_ffi.lib().tok_adam_master_step(
-            C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], beta1, beta2,
-            group["eps"], group["weight_decay"], int(group["decoupled_weight_decay"]),
-            int(group["amsgrad"]), step, C.c_void_p(stream.cuda_stream)))
+        args = [C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], beta1, beta2,
+                group["eps"], group["weight_decay"], int(group["decoupled_weight_decay"]),
+                int(group["amsgrad"]), step]
+        if coef is None:
+            _ffi.check(_ffi.lib().tok_adam_master_step(*args, C.c_void_p(stream.cuda_stream)))
+        else:
+            _ffi.check(_ffi.lib().tok_adam_master_step_clipped(
+                *args, C.c_void_p(coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
 
 
 class MasterWeightAdamW(MasterWeightAdam):
@@ -303,7 +462,9 @@ class MasterWeightAdamW(MasterWeightAdam):
     def __init__(self, params, lr: float = 1e-3, betas: Tuple[float, float] = (0.9, 0.999),
                  eps: float = 1e-8, weight_decay: float = 1e-2, amsgrad: bool = False, *,
                  maximize: bool = False, foreach: Optional[bool] = None, capturable: bool = False,
-                 differentiable: bool = False, fused: Optional[bool] = None):
+                 differentiable: bool = False, fused: Optional[bool] = None,
+                 max_grad_norm: Optional[float] = None, error_if_nonfinite: bool = False):
         super().__init__(params, lr, betas, eps, weight_decay, amsgrad, foreach=foreach,
                          maximize=maximize, capturable=capturable, differentiable=differentiable,
-                         fused=fused, decoupled_weight_decay=True)
+                         fused=fused, decoupled_weight_decay=True, max_grad_norm=max_grad_norm,
+                         error_if_nonfinite=error_if_nonfinite)

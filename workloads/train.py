@@ -41,6 +41,9 @@ def main() -> int:
                          "MasterWeightAdamW with --optimizer adamw)")
     ap.add_argument("--optimizer", choices=("sgd", "adamw"), default="sgd",
                     help="sgd: lr 0.01, momentum 0.9; adamw: torch.optim.AdamW's defaults")
+    ap.add_argument("--clip-grad-norm", type=float, default=None, metavar="X",
+                    help="clip the global gradient L2 norm at X: max_grad_norm=X with "
+                         "--master-weights, else torch.nn.utils.clip_grad_norm_ before opt.step()")
     a = ap.parse_args()
 
     import torch
@@ -54,8 +57,10 @@ def main() -> int:
         model = model.to(memory_format=torch.channels_last)
     if a.master_weights:
         from torch_on_k8s_b200.optim import MasterWeightAdamW, MasterWeightSGD
-        opt = MasterWeightAdamW(model.parameters()) if a.optimizer == "adamw" else \
-            MasterWeightSGD(model.parameters(), lr=0.01, momentum=0.9)
+        opt = MasterWeightAdamW(model.parameters(), max_grad_norm=a.clip_grad_norm) \
+            if a.optimizer == "adamw" else \
+            MasterWeightSGD(model.parameters(), lr=0.01, momentum=0.9,
+                            max_grad_norm=a.clip_grad_norm)
         ddp, hook = rep.wrap(model, record_events=(rep.rank == 0), optimizer=opt)
     else:
         ddp, hook = rep.wrap(model, record_events=(rep.rank == 0))
@@ -73,7 +78,13 @@ def main() -> int:
         out = ddp(x).float()
         loss = torch.nn.functional.cross_entropy(out, y)
         loss.backward()
+        grad_norm = None
+        if a.clip_grad_norm is not None and not a.master_weights:
+            # after backward: DDP's hook has averaged the gradients by now
+            grad_norm = torch.nn.utils.clip_grad_norm_(ddp.parameters(), a.clip_grad_norm)
         opt.step()
+        if a.clip_grad_norm is not None and a.master_weights:
+            grad_norm = opt.grad_norm
         if (step + 1) % a.log_every == 0 and rep.rank <= 1:
             torch.cuda.synchronize()
             now = time.time()
@@ -82,7 +93,8 @@ def main() -> int:
             acc = float((out.argmax(1) == y).float().mean()) * 100
             print("Epoch: [0][%4d/%d]\tTime %6.3f (%6.3f)\tData  0.000 ( 0.000)\tLoss %.4e\t"
                   "Acc@1 %6.2f (%6.2f)\tAcc@5 %6.2f (%6.2f)" %
-                  (step + 1, a.steps, lat, lat, float(loss), acc, acc, acc, acc), flush=True)
+                  (step + 1, a.steps, lat, lat, float(loss), acc, acc, acc, acc) +
+                  ("" if grad_norm is None else "\tGradNorm %.4e" % float(grad_norm)), flush=True)
             if rep.rank == 0 and rep.world > 1:
                 ev = hook.drain_events()       # [(wire bytes, bucket bytes, exchange ms, wait ms)]
                 ms = sum(e[2] for e in ev)

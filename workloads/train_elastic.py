@@ -63,6 +63,10 @@ def main() -> int:
                          "with --optimizer adamw)")
     ap.add_argument("--optimizer", choices=("sgd", "adamw"), default="sgd",
                     help="sgd: momentum 0.9; adamw: torch.optim.AdamW's defaults but --lr")
+    ap.add_argument("--clip-grad-norm", type=float, default=None, metavar="X",
+                    help="clip the global gradient L2 norm at X: max_grad_norm=X with "
+                         "--master-weights, else torch.nn.utils.clip_grad_norm_ between the "
+                         "exchange and opt.step()")
     a = ap.parse_args()
 
     t_proc = time.time()
@@ -84,8 +88,10 @@ def main() -> int:
     edp = ElasticDataParallel(model, rep.comm, bucket_cap_mb=25)
     if a.master_weights:
         from torch_on_k8s_b200.optim import MasterWeightAdamW, MasterWeightSGD
-        opt = MasterWeightAdamW(model.parameters(), lr=a.lr) if a.optimizer == "adamw" else \
-            MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9)
+        opt = MasterWeightAdamW(model.parameters(), lr=a.lr, max_grad_norm=a.clip_grad_norm) \
+            if a.optimizer == "adamw" else \
+            MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9,
+                            max_grad_norm=a.clip_grad_norm)
     else:
         opt = torch.optim.AdamW(model.parameters(), lr=a.lr) if a.optimizer == "adamw" else \
             torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
@@ -129,13 +135,19 @@ def main() -> int:
         loss = loss_of(edp)
         loss.backward()
         edp.reduce_grads(optimizer=opt if a.master_weights else None)
+        grad_norm = None
+        if a.clip_grad_norm is not None and not a.master_weights:
+            grad_norm = torch.nn.utils.clip_grad_norm_(model.parameters(), a.clip_grad_norm)
         opt.step()
+        if a.clip_grad_norm is not None and a.master_weights:
+            grad_norm = opt.grad_norm
         torch.cuda.synchronize()
         now = time.time()
         dt, t_prev = now - t_prev, now
         step += 1
         lat_acc.append(dt)
-        log(event="step", step=step, seconds=dt, units=units, loss=float(loss))
+        log(event="step", step=step, seconds=dt, units=units, loss=float(loss),
+            **({} if grad_norm is None else dict(grad_norm=float(grad_norm))))
         if step % a.log_every == 0 and rep.rank <= 1:
             lat = sum(lat_acc) / len(lat_acc)
             lat_acc = []
