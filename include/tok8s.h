@@ -316,6 +316,25 @@ int tok_adam_master_step_clipped(const tok_adam_segment_t* segments, int count, 
                                  double weight_decay, int decoupled, int amsgrad, double step,
                                  const float* grad_coef, void* cuda_stream);
 
+/* tok_sgd_master_step / tok_adam_master_step with dynamic loss scaling: the same step, table and
+ * rules, with grad = f32(segment.grad) * *inv_scale (one rounding) as the master's gradient — the bits
+ * torch.amp.GradScaler.unscale_ (_amp_foreach_non_finite_check_and_unscale_) stores in master.grad.
+ * When `grad_coef` is not NULL, grad = grad * *grad_coef follows as a second rounding, the bits of
+ * clip_grad_norm_ multiplying the unscaled master.grad; the two multiplies are not folded into one,
+ * which would differ whenever *inv_scale is not a power of two.  `inv_scale` and `grad_coef` are
+ * DEVICE fp32 scalars read by the kernel.  The caller launches these only when no gradient was inf or
+ * NaN (tok_grad_nonfinite), as GradScaler.step skips the step otherwise.  Returns what the plain
+ * entry point returns, and TOK_ERR_INVALID for a null `inv_scale`. */
+int tok_sgd_master_step_unscaled(const tok_sgd_segment_t* segments, int count, int64_t chunks,
+                                 int dtype, double lr, double momentum, double dampening,
+                                 double weight_decay, int nesterov, int fresh,
+                                 const float* inv_scale, const float* grad_coef, void* cuda_stream);
+int tok_adam_master_step_unscaled(const tok_adam_segment_t* segments, int count, int64_t chunks,
+                                  int dtype, double lr, double beta1, double beta2, double eps,
+                                  double weight_decay, int decoupled, int amsgrad, double step,
+                                  const float* inv_scale, const float* grad_coef,
+                                  void* cuda_stream);
+
 /* Per-tensor L2 norms of bf16 / f16 gradients (gradient clipping in torch_on_k8s_b200/optim.py): for
  * every segment, norms[slot] receives the bits of torch._foreach_norm([f32(grad)], 2)[0] — ATen's
  * chunking, per-thread accumulators, FMA squares, block reduction trees and correctly rounded sqrt,
@@ -336,6 +355,30 @@ typedef struct tok_norm_segment {
 } tok_norm_segment_t;
 int tok_grad_norms(const tok_norm_segment_t* segments, int count, int64_t chunks, int dtype,
                    float* partials, float* norms, void* cuda_stream);
+
+/* tok_grad_norms for dynamic loss scaling: norms[slot] receives the bits of
+ * torch._foreach_norm([f32(grad) * *inv_scale], 2)[0], each element unscaled with one rounding before
+ * its square (the master.grad GradScaler.unscale_ leaves), and *found_inf is set to 1.0f when any raw
+ * element of any segment is inf or NaN — in the same pass, so clipping with loss scaling reads each
+ * gradient once.  `found_inf` is only ever written with 1.0f: the caller zeroes it once per iteration.
+ * The table, `partials` and `norms` follow tok_grad_norms's rules.  Two launches.  Returns what
+ * tok_grad_norms returns, and TOK_ERR_INVALID for a null `inv_scale` or `found_inf`. */
+int tok_grad_norms_unscaled(const tok_norm_segment_t* segments, int count, int64_t chunks,
+                            int dtype, const float* inv_scale, float* partials, float* norms,
+                            float* found_inf, void* cuda_stream);
+
+/* The inf / NaN check of dynamic loss scaling (torch_on_k8s_b200/optim.py's loss_scale): writes
+ * *found_inf = 1.0f when any element of any segment is inf or NaN and writes nothing otherwise, the
+ * verdict of _amp_foreach_non_finite_check_and_unscale_ on f32(grad).  The table is
+ * tok_grad_norms's (TOK_NORM_CHUNK elements per chunk, one CTA per chunk, a DEVICE array; `slot` is
+ * unused).  Only the segments' elements are read: nothing between or around them.  16-byte loads
+ * where the view is aligned, scalar loads for its head and tail, at most one store per CTA.  The
+ * caller zeroes `found_inf` once per iteration, as GradScaler creates found_inf = 0.  One launch, none
+ * when `chunks` is 0.  Returns TOK_ERR_INVALID for a null table or `found_inf`, an empty table, a
+ * negative or too large `chunks`, a dtype other than TOK_BF16 / TOK_F16, TOK_ERR_NO_DEVICE without a
+ * GPU.  Enqueued on `cuda_stream`, no synchronisation. */
+int tok_grad_nonfinite(const tok_norm_segment_t* segments, int count, int64_t chunks, int dtype,
+                       float* found_inf, void* cuda_stream);
 
 /* Which algorithm AUTO picks for `wire_bytes` on this communicator. */
 int tok_allreduce_algo(tok_comm_t* comm, size_t wire_bytes, int* algo);

@@ -51,6 +51,14 @@
 // tensor clip_grad_norm_ forms on the device (grad_norm.cu computes the norms it is formed from).  The
 // unclipped instantiations compile to the SASS they had before the flag existed.
 //
+// Unscaled steps (tok_*_master_step_unscaled, dynamic loss scaling) add kUnscale: the first operation
+// becomes g = f32(grad) * inv_scale, one rounding, as torch's _amp_foreach_non_finite_check_and_unscale_
+// stores master.grad (its `inv_scale == 1 ? val : val * inv_scale` is the same bits for every value it
+// does not flag as non-finite).  With a clip coefficient as well, g = g * coef follows as a second
+// rounding: GradScaler.unscale_ and clip_grad_norm_ each store master.grad, and one multiply by
+// inv_scale * coef would differ whenever inv_scale is not a power of two.  The plain and clipped
+// instantiations compile to the SASS they had before this flag existed.
+//
 // Both kernels split work over (segment, chunk) pairs: block b takes chunk b of the whole table and
 // finds its segment by binary search over the entries' first-chunk indices.  Inside a chunk, 8
 // elements at a time go through 16-byte vector loads and stores where the parameter and every fp32
@@ -122,22 +130,25 @@ __device__ __forceinline__ void store_param8(void* param, int64_t i, const uint1
                  out[4] | ((uint32_t)out[5] << 16), out[6] | ((uint32_t)out[7] << 16));
 }
 
-// The gradient element as the optimizer reads it: f32(grad), and with kClip that times the clip
+// The gradient element as the optimizer reads it: f32(grad); with kUnscale that times the inverse loss
+// scale, rounded once, as GradScaler.unscale_ stores master.grad; with kClip that times the clip
 // coefficient, rounded once, as torch's clip_grad_norm_ multiplies master.grad (_foreach_mul_) before
 // the optimizer step reads it.
-template <typename T, bool kClip>
-__device__ __forceinline__ float grad_in(uint16_t bits, float coef) {
-  return kClip ? __fmul_rn(widen<T>(bits), coef) : widen<T>(bits);
+template <typename T, bool kClip, bool kUnscale>
+__device__ __forceinline__ float grad_in(uint16_t bits, float coef, float inv_scale) {
+  const float g = kUnscale ? __fmul_rn(widen<T>(bits), inv_scale) : widen<T>(bits);
+  return kClip ? __fmul_rn(g, coef) : g;
 }
 
 // Chunk blockIdx.x of the table in `a` (a Step: SgdArgs or AdamArgs).  Thread 0 finds the last entry
 // whose first chunk is <= the block's and copies it to shared memory; then the block walks the
 // chunk's elements: Step::vector for 8 at a time from the first element at which the parameter is
 // 16-byte aligned, if Step::vectorizable says every fp32 array is aligned there too, and
-// Step::scalar for the rest.  With kClip, every gradient element is multiplied by `coef` (the clip
-// coefficient) before anything else reads it; without, `coef` is unused.
-template <typename T, bool kClip, typename Step>
-__device__ __forceinline__ void walk_chunk(const Step& a, float coef) {
+// Step::scalar for the rest.  With kUnscale, every gradient element is multiplied by `inv_scale` (the
+// inverse loss scale) before anything else reads it, and with kClip then by `coef` (the clip
+// coefficient); without the flags, those arguments are unused.
+template <typename T, bool kClip, bool kUnscale, typename Step>
+__device__ __forceinline__ void walk_chunk(const Step& a, float coef, float inv_scale) {
   __shared__ typename Step::Segment s;
   const int64_t c = blockIdx.x;
   if (threadIdx.x == 0) {
@@ -159,10 +170,11 @@ __device__ __forceinline__ void walk_chunk(const Step& a, float coef) {
   const int64_t vbeg = start + head, tail = vbeg + 8 * nvec;
   const bool grad_vec = aligned16(s.grad, vbeg, 2);
   for (int64_t v = threadIdx.x; v < nvec; v += kSgdThreads)
-    a.template vector<T, kClip>(s, vbeg + 8 * v, grad_vec, coef);
+    a.template vector<T, kClip, kUnscale>(s, vbeg + 8 * v, grad_vec, coef, inv_scale);
   const int64_t nscalar = head + (end - tail);
   for (int64_t j = threadIdx.x; j < nscalar; j += kSgdThreads)
-    a.template scalar<T, kClip>(s, j < head ? start + j : tail + (j - head), coef);
+    a.template scalar<T, kClip, kUnscale>(s, j < head ? start + j : tail + (j - head), coef,
+                                          inv_scale);
 }
 
 // ---- SGD ----------------------------------------------------------------------------------------
@@ -193,9 +205,10 @@ struct SgdArgs {
     return aligned16(s.master, i, 4) && (!use_mu || aligned16(s.momentum, i, 4));
   }
 
-  template <typename T, bool kClip>
-  __device__ __forceinline__ void scalar(const tok_sgd_segment_t& s, int64_t i, float coef) const {
-    const float g = grad_in<T, kClip>(__ldg((const uint16_t*)s.grad + i), coef);
+  template <typename T, bool kClip, bool kUnscale>
+  __device__ __forceinline__ void scalar(const tok_sgd_segment_t& s, int64_t i, float coef,
+                                         float inv_scale) const {
+    const float g = grad_in<T, kClip, kUnscale>(__ldg((const uint16_t*)s.grad + i), coef, inv_scale);
     float m = (use_mu && !fresh) ? s.momentum[i] : 0.0f;
     const float w = step(g, s.master[i], m);
     s.master[i] = w;
@@ -203,9 +216,9 @@ struct SgdArgs {
     ((uint16_t*)s.param)[i] = narrow<T>(w);
   }
 
-  template <typename T, bool kClip>
+  template <typename T, bool kClip, bool kUnscale>
   __device__ __forceinline__ void vector(const tok_sgd_segment_t& s, int64_t i, bool grad_vec,
-                                         float coef) const {
+                                         float coef, float inv_scale) const {
     // The gradient load is load_grad8 written out: called through the helper, ptxas schedules this
     // kernel differently (46 registers instead of 48); written out, its SASS is what it was before
     // the Adam kernel shared this file.
@@ -235,7 +248,8 @@ struct SgdArgs {
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       m[k] = k < 4 ? lane(m0, k) : lane(m1, k - 4);
-      w[k] = step(grad_in<T, kClip>(gb[k], coef), k < 4 ? lane(w0, k) : lane(w1, k - 4), m[k]);
+      w[k] = step(grad_in<T, kClip, kUnscale>(gb[k], coef, inv_scale),
+                  k < 4 ? lane(w0, k) : lane(w1, k - 4), m[k]);
       out[k] = narrow<T>(w[k]);
     }
     wp[0] = make_float4(w[0], w[1], w[2], w[3]);
@@ -250,13 +264,20 @@ struct SgdArgs {
 
 template <typename T>
 __global__ void __launch_bounds__(kSgdThreads) sgd_master_kernel(const SgdArgs a) {
-  walk_chunk<T, false>(a, 1.0f);
+  walk_chunk<T, false, false>(a, 1.0f, 1.0f);
 }
 
 template <typename T>
 __global__ void __launch_bounds__(kSgdThreads)
     sgd_master_clipped_kernel(const SgdArgs a, const float* __restrict__ grad_coef) {
-  walk_chunk<T, true>(a, __ldg(grad_coef));
+  walk_chunk<T, true, false>(a, __ldg(grad_coef), 1.0f);
+}
+
+template <typename T, bool kClip>
+__global__ void __launch_bounds__(kSgdThreads)
+    sgd_master_unscaled_kernel(const SgdArgs a, const float* __restrict__ inv_scale,
+                               const float* __restrict__ grad_coef) {
+  walk_chunk<T, kClip, true>(a, kClip ? __ldg(grad_coef) : 1.0f, __ldg(inv_scale));
 }
 
 // ---- Adam / AdamW -------------------------------------------------------------------------------
@@ -303,9 +324,10 @@ struct AdamArgs {
            aligned16(s.exp_avg_sq, i, 4) && (!amsgrad || aligned16(s.max_exp_avg_sq, i, 4));
   }
 
-  template <typename T, bool kClip>
-  __device__ __forceinline__ void scalar(const tok_adam_segment_t& s, int64_t i, float coef) const {
-    const float g = grad_in<T, kClip>(__ldg((const uint16_t*)s.grad + i), coef);
+  template <typename T, bool kClip, bool kUnscale>
+  __device__ __forceinline__ void scalar(const tok_adam_segment_t& s, int64_t i, float coef,
+                                         float inv_scale) const {
+    const float g = grad_in<T, kClip, kUnscale>(__ldg((const uint16_t*)s.grad + i), coef, inv_scale);
     float m = s.exp_avg[i], v = s.exp_avg_sq[i];
     float vmax = amsgrad ? s.max_exp_avg_sq[i] : 0.0f;
     const float w = step(g, s.master[i], m, v, vmax);
@@ -316,9 +338,9 @@ struct AdamArgs {
     ((uint16_t*)s.param)[i] = narrow<T>(w);
   }
 
-  template <typename T, bool kClip>
+  template <typename T, bool kClip, bool kUnscale>
   __device__ __forceinline__ void vector(const tok_adam_segment_t& s, int64_t i, bool grad_vec,
-                                         float coef) const {
+                                         float coef, float inv_scale) const {
     uint16_t gb[8];
     load_grad8(s.grad, i, grad_vec, gb);
     float4* wp = (float4*)(s.master + i);
@@ -338,8 +360,8 @@ struct AdamArgs {
       m[k] = k < 4 ? lane(m0, k) : lane(m1, k - 4);
       v[k] = k < 4 ? lane(v0, k) : lane(v1, k - 4);
       x[k] = k < 4 ? lane(x0, k) : lane(x1, k - 4);
-      w[k] = step(grad_in<T, kClip>(gb[k], coef), k < 4 ? lane(w0, k) : lane(w1, k - 4), m[k],
-                  v[k], x[k]);
+      w[k] = step(grad_in<T, kClip, kUnscale>(gb[k], coef, inv_scale),
+                  k < 4 ? lane(w0, k) : lane(w1, k - 4), m[k], v[k], x[k]);
       out[k] = narrow<T>(w[k]);
     }
     wp[0] = make_float4(w[0], w[1], w[2], w[3]);
@@ -358,13 +380,20 @@ struct AdamArgs {
 
 template <typename T>
 __global__ void __launch_bounds__(kSgdThreads) adam_master_kernel(const AdamArgs a) {
-  walk_chunk<T, false>(a, 1.0f);
+  walk_chunk<T, false, false>(a, 1.0f, 1.0f);
 }
 
 template <typename T>
 __global__ void __launch_bounds__(kSgdThreads)
     adam_master_clipped_kernel(const AdamArgs a, const float* __restrict__ grad_coef) {
-  walk_chunk<T, true>(a, __ldg(grad_coef));
+  walk_chunk<T, true, false>(a, __ldg(grad_coef), 1.0f);
+}
+
+template <typename T, bool kClip>
+__global__ void __launch_bounds__(kSgdThreads)
+    adam_master_unscaled_kernel(const AdamArgs a, const float* __restrict__ inv_scale,
+                                const float* __restrict__ grad_coef) {
+  walk_chunk<T, kClip, true>(a, kClip ? __ldg(grad_coef) : 1.0f, __ldg(inv_scale));
 }
 
 // The table and dtype checks both entry points share; 0 when they pass.
@@ -383,11 +412,12 @@ int launched(const char* who) {
   return TOK_OK;
 }
 
-// The SGD entry points: checks, the float hyperparameters, and one launch of the plain kernel or,
-// with a coefficient, the clipped one.
+// The SGD entry points: checks, the float hyperparameters, and one launch of the plain kernel, with a
+// coefficient the clipped one, or with `unscale` the unscaled one (clipped too when grad_coef is set).
 int sgd_step(const char* who, const tok_sgd_segment_t* segments, int count, int64_t chunks,
              int dtype, double lr, double momentum, double dampening, double weight_decay,
-             int nesterov, int fresh, const float* grad_coef, bool clip, void* cuda_stream) {
+             int nesterov, int fresh, const float* grad_coef, bool clip, const float* inv_scale,
+             bool unscale, void* cuda_stream) {
   if (const int rc = check_table(who, segments, count, chunks, dtype)) return rc;
   if (!(lr >= 0.0) || !isfinite(lr)) return fail(TOK_ERR_INVALID, "%s: lr %g", who, lr);
   if (!(momentum >= 0.0) || !isfinite(momentum))
@@ -398,6 +428,7 @@ int sgd_step(const char* who, const tok_sgd_segment_t* segments, int count, int6
   if (nesterov && (momentum <= 0.0 || dampening != 0.0))
     return fail(TOK_ERR_INVALID, "%s: nesterov needs a momentum and zero dampening", who);
   if (clip && !grad_coef) return fail(TOK_ERR_INVALID, "%s: null grad_coef", who);
+  if (unscale && !inv_scale) return fail(TOK_ERR_INVALID, "%s: null inv_scale", who);
   if (!device_ready()) return fail(TOK_ERR_NO_DEVICE, "%s needs a CUDA GPU (no CPU fallback)", who);
   SgdArgs a{};
   a.seg = segments;
@@ -412,7 +443,19 @@ int sgd_step(const char* who, const tok_sgd_segment_t* segments, int count, int6
   a.fresh = fresh != 0;
   const dim3 grid((unsigned)chunks);
   const cudaStream_t st = (cudaStream_t)cuda_stream;
-  if (clip) {
+  if (unscale) {
+    if (dtype == TOK_BF16 && grad_coef)
+      sgd_master_unscaled_kernel<__nv_bfloat16, true><<<grid, kSgdThreads, 0, st>>>(a, inv_scale,
+                                                                                   grad_coef);
+    else if (dtype == TOK_BF16)
+      sgd_master_unscaled_kernel<__nv_bfloat16, false><<<grid, kSgdThreads, 0, st>>>(a, inv_scale,
+                                                                                    grad_coef);
+    else if (grad_coef)
+      sgd_master_unscaled_kernel<__half, true><<<grid, kSgdThreads, 0, st>>>(a, inv_scale, grad_coef);
+    else
+      sgd_master_unscaled_kernel<__half, false><<<grid, kSgdThreads, 0, st>>>(a, inv_scale,
+                                                                             grad_coef);
+  } else if (clip) {
     if (dtype == TOK_BF16)
       sgd_master_clipped_kernel<__nv_bfloat16><<<grid, kSgdThreads, 0, st>>>(a, grad_coef);
     else
@@ -429,7 +472,7 @@ int sgd_step(const char* who, const tok_sgd_segment_t* segments, int count, int6
 int adam_step(const char* who, const tok_adam_segment_t* segments, int count, int64_t chunks,
               int dtype, double lr, double beta1, double beta2, double eps, double weight_decay,
               int decoupled, int amsgrad, double step, const float* grad_coef, bool clip,
-              void* cuda_stream) {
+              const float* inv_scale, bool unscale, void* cuda_stream) {
   if (const int rc = check_table(who, segments, count, chunks, dtype)) return rc;
   if (!(lr >= 0.0) || !isfinite(lr)) return fail(TOK_ERR_INVALID, "%s: lr %g", who, lr);
   if (!(beta1 >= 0.0 && beta1 < 1.0))
@@ -441,6 +484,7 @@ int adam_step(const char* who, const tok_adam_segment_t* segments, int count, in
     return fail(TOK_ERR_INVALID, "%s: weight_decay %g", who, weight_decay);
   if (!(step >= 1.0) || !isfinite(step)) return fail(TOK_ERR_INVALID, "%s: step %g", who, step);
   if (clip && !grad_coef) return fail(TOK_ERR_INVALID, "%s: null grad_coef", who);
+  if (unscale && !inv_scale) return fail(TOK_ERR_INVALID, "%s: null inv_scale", who);
   if (!device_ready()) return fail(TOK_ERR_NO_DEVICE, "%s needs a CUDA GPU (no CPU fallback)", who);
   // torch's Python, in double: bias_correction1 = 1 - beta1 ** step; step_size = (lr / bc1) * -1;
   // bias_correction2_sqrt = (1 - beta2 ** step) ** 0.5 — CPython's float ** is libm's pow
@@ -461,7 +505,20 @@ int adam_step(const char* who, const tok_adam_segment_t* segments, int count, in
   a.amsgrad = amsgrad != 0;
   const dim3 grid((unsigned)chunks);
   const cudaStream_t st = (cudaStream_t)cuda_stream;
-  if (clip) {
+  if (unscale) {
+    if (dtype == TOK_BF16 && grad_coef)
+      adam_master_unscaled_kernel<__nv_bfloat16, true><<<grid, kSgdThreads, 0, st>>>(a, inv_scale,
+                                                                                    grad_coef);
+    else if (dtype == TOK_BF16)
+      adam_master_unscaled_kernel<__nv_bfloat16, false><<<grid, kSgdThreads, 0, st>>>(a, inv_scale,
+                                                                                     grad_coef);
+    else if (grad_coef)
+      adam_master_unscaled_kernel<__half, true><<<grid, kSgdThreads, 0, st>>>(a, inv_scale,
+                                                                             grad_coef);
+    else
+      adam_master_unscaled_kernel<__half, false><<<grid, kSgdThreads, 0, st>>>(a, inv_scale,
+                                                                              grad_coef);
+  } else if (clip) {
     if (dtype == TOK_BF16)
       adam_master_clipped_kernel<__nv_bfloat16><<<grid, kSgdThreads, 0, st>>>(a, grad_coef);
     else
@@ -484,7 +541,7 @@ extern "C" int tok_sgd_master_step(const tok_sgd_segment_t* segments, int count,
                                    double weight_decay, int nesterov, int fresh,
                                    void* cuda_stream) {
   return sgd_step("tok_sgd_master_step", segments, count, chunks, dtype, lr, momentum, dampening,
-                  weight_decay, nesterov, fresh, nullptr, false, cuda_stream);
+                  weight_decay, nesterov, fresh, nullptr, false, nullptr, false, cuda_stream);
 }
 
 extern "C" int tok_sgd_master_step_clipped(const tok_sgd_segment_t* segments, int count,
@@ -492,7 +549,18 @@ extern "C" int tok_sgd_master_step_clipped(const tok_sgd_segment_t* segments, in
                                            double dampening, double weight_decay, int nesterov,
                                            int fresh, const float* grad_coef, void* cuda_stream) {
   return sgd_step("tok_sgd_master_step_clipped", segments, count, chunks, dtype, lr, momentum,
-                  dampening, weight_decay, nesterov, fresh, grad_coef, true, cuda_stream);
+                  dampening, weight_decay, nesterov, fresh, grad_coef, true, nullptr, false,
+                  cuda_stream);
+}
+
+extern "C" int tok_sgd_master_step_unscaled(const tok_sgd_segment_t* segments, int count,
+                                            int64_t chunks, int dtype, double lr, double momentum,
+                                            double dampening, double weight_decay, int nesterov,
+                                            int fresh, const float* inv_scale,
+                                            const float* grad_coef, void* cuda_stream) {
+  return sgd_step("tok_sgd_master_step_unscaled", segments, count, chunks, dtype, lr, momentum,
+                  dampening, weight_decay, nesterov, fresh, grad_coef, false, inv_scale, true,
+                  cuda_stream);
 }
 
 extern "C" int tok_adam_master_step(const tok_adam_segment_t* segments, int count, int64_t chunks,
@@ -500,7 +568,8 @@ extern "C" int tok_adam_master_step(const tok_adam_segment_t* segments, int coun
                                     double weight_decay, int decoupled, int amsgrad, double step,
                                     void* cuda_stream) {
   return adam_step("tok_adam_master_step", segments, count, chunks, dtype, lr, beta1, beta2, eps,
-                   weight_decay, decoupled, amsgrad, step, nullptr, false, cuda_stream);
+                   weight_decay, decoupled, amsgrad, step, nullptr, false, nullptr, false,
+                   cuda_stream);
 }
 
 extern "C" int tok_adam_master_step_clipped(const tok_adam_segment_t* segments, int count,
@@ -509,6 +578,17 @@ extern "C" int tok_adam_master_step_clipped(const tok_adam_segment_t* segments, 
                                             int decoupled, int amsgrad, double step,
                                             const float* grad_coef, void* cuda_stream) {
   return adam_step("tok_adam_master_step_clipped", segments, count, chunks, dtype, lr, beta1,
-                   beta2, eps, weight_decay, decoupled, amsgrad, step, grad_coef, true,
-                   cuda_stream);
+                   beta2, eps, weight_decay, decoupled, amsgrad, step, grad_coef, true, nullptr,
+                   false, cuda_stream);
+}
+
+extern "C" int tok_adam_master_step_unscaled(const tok_adam_segment_t* segments, int count,
+                                             int64_t chunks, int dtype, double lr, double beta1,
+                                             double beta2, double eps, double weight_decay,
+                                             int decoupled, int amsgrad, double step,
+                                             const float* inv_scale, const float* grad_coef,
+                                             void* cuda_stream) {
+  return adam_step("tok_adam_master_step_unscaled", segments, count, chunks, dtype, lr, beta1,
+                   beta2, eps, weight_decay, decoupled, amsgrad, step, grad_coef, false, inv_scale,
+                   true, cuda_stream);
 }

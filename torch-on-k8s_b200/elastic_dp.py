@@ -93,7 +93,9 @@ class ElasticDataParallel(torch.nn.Module):
         optimizer (a MasterWeightSGD, MasterWeightAdam or MasterWeightAdamW): each bucket's step is
         enqueued right behind its exchange; optimizer.step() then launches nothing for these
         parameters.  With max_grad_norm only the bucket's gradient norms are enqueued there, and
-        optimizer.step() steps every bucket once the global norm exists."""
+        optimizer.step() steps every bucket once the global norm exists.  With a loss scale only the
+        bucket's inf / NaN check (or its unscaled norms) is enqueued there, and optimizer.step()
+        steps every bucket unless an inf or NaN was found."""
         world = self.comm.world
         for k, b in enumerate(self.buckets):   # PRE scale: the same function as built-in DDP
             self.comm.allreduce_bucket(b, b, scale=1.0 / world, algo=self.algo, stream=stream)
@@ -107,10 +109,13 @@ class ElasticDataParallel(torch.nn.Module):
 
     def hand_over(self, optimizer: torch.optim.Optimizer, step: int, root: int = 0) -> int:
         """What every member runs right after a re-form or a join, before its next step: `root`'s
-        parameters, buffers, optimizer state and step counter to the whole group, in this order on
-        every replica, then a device synchronize.  Returns `root`'s step."""
+        parameters, buffers, optimizer state, loss scale (when the optimizer has one) and step
+        counter to the whole group, in this order on every replica, then a device synchronize.
+        Returns `root`'s step."""
         self.sync_params(root)
         self.sync_optimizer_state(optimizer, root)
+        if getattr(optimizer, "loss_scale", None) is not None:
+            self.sync_loss_scale(optimizer.loss_scale, root)
         cell = torch.zeros(2, dtype=torch.int64, device=next(self.module.parameters()).device)
         cell[0] = step
         self.comm.broadcast(cell, root)
@@ -125,6 +130,18 @@ class ElasticDataParallel(torch.nn.Module):
         self.comm.broadcast_coalesced([p.data for p in self.module.parameters()] +
                                       [b for b in self.module.buffers()], root,
                                       use_pool=self.pool_broadcast)
+
+    @torch.no_grad()
+    def sync_loss_scale(self, loss_scale, root: int = 0) -> None:
+        """Replicate `root`'s dynamic loss scale and growth tracker (one 8-byte broadcast).  Without
+        it a joiner would scale its loss by init_scale while the others use their current scale, and
+        the averaged gradient would mix the two."""
+        loss_scale._ensure(next(self.module.parameters()).device)
+        cell = torch.stack([loss_scale.scale_tensor.view(torch.int32), loss_scale.growth_tracker])
+        self.comm.broadcast(cell, root)
+        loss_scale.scale_tensor.copy_(cell[0].view(torch.float32))
+        loss_scale.growth_tracker.copy_(cell[1])
+        loss_scale._refresh()
 
     @torch.no_grad()
     def sync_optimizer_state(self, optimizer: torch.optim.Optimizer, root: int = 0) -> None:

@@ -38,6 +38,32 @@ every gradient, so each bucket's hook only enqueues its per-tensor norms (csrc/g
 its exchange; step() forms the total and the coefficient with clip_grad_norm_'s own torch
 expressions on the device and launches every bucket's clipped step then.  Clipping thus moves the
 steps from behind each exchange to after backward.  Norm types other than 2 are not supported.
+
+Dynamic loss scaling.  f16 gradients below about 6e-8 flush to zero and above 65504 overflow, so f16
+training multiplies the loss by a dynamic scale.  torch.amp.GradScaler cannot drive these optimizers:
+their param_groups hold f16 parameters, which GradScaler refuses to unscale, and an overlapped
+optimizer has stepped every bucket with still-scaled gradients before any scaler could look at them.
+Pass `loss_scale=DynamicLossScale(...)` instead and run
+
+    opt.loss_scale.scale(loss).backward()
+    opt.step()
+
+One iteration then gives the bits of the stock loop on fp32 masters
+
+    scaler.scale(loss).backward()
+    for each master: master.grad = p.grad.float()       (None where p.grad is None)
+    scaler.unscale_(opt)                                 # unscale and check for inf / NaN
+    total = clip_grad_norm_(masters, c)                  # only with max_grad_norm=c
+    scaler.step(opt)                                     # skipped when an inf or NaN was found
+    scaler.update()
+    p.copy_(master)                                      # only when the step ran
+
+including the scale and growth tracker.  Each bucket's hook enqueues only its inf / NaN check
+(csrc/grad_norm.cu), or with clipping its unscaled norms, which set the same flag; step() reads the
+flag on the host once, as GradScaler.step does, launches every unscaled step when it is clear, and
+updates the scale with torch._amp_update_scale_.  `opt.found_inf` (a device tensor) and
+`opt.step_skipped` (a bool) tell what the last step() did.  No collective is needed: every replica
+holds the same averaged gradients and so reaches the same verdict and the same scale.
 """
 from __future__ import annotations
 
@@ -98,6 +124,93 @@ def _check_max_grad_norm(max_grad_norm) -> Optional[float]:
     return float(max_grad_norm)
 
 
+class DynamicLossScale:
+    """torch.amp.GradScaler's dynamic loss scale for the master-weight optimizers' `loss_scale=`.
+
+    It holds a 0-d fp32 `scale_tensor`, an int32 `growth_tracker` and `inv_scale`, formed with
+    GradScaler's own expression, all on the device of the first loss it scales (or of the first
+    gradients the optimizer checks).  state_dict() and load_state_dict() use GradScaler's keys, so a
+    checkpoint moves either way between this and a stock GradScaler."""
+
+    def __init__(self, init_scale: float = 2.0 ** 16, growth_factor: float = 2.0,
+                 backoff_factor: float = 0.5, growth_interval: int = 2000):
+        # GradScaler's checks and messages, then what GradScaler would accept but cannot work
+        if growth_factor <= 1.0:
+            raise ValueError("The growth factor must be > 1.0.")
+        if backoff_factor >= 1.0:
+            raise ValueError("The backoff factor must be < 1.0.")
+        if isinstance(init_scale, bool) or not isinstance(init_scale, (int, float)) or \
+                not math.isfinite(init_scale) or init_scale <= 0:
+            raise ValueError("init_scale must be a finite number > 0, got %r" % (init_scale,))
+        if isinstance(growth_interval, bool) or not isinstance(growth_interval, int) or \
+                growth_interval < 1:
+            raise ValueError("growth_interval must be an int >= 1, got %r" % (growth_interval,))
+        self._init_scale = float(init_scale)
+        self._init_growth_tracker = 0
+        self.growth_factor = float(growth_factor)
+        self.backoff_factor = float(backoff_factor)
+        self.growth_interval = growth_interval
+        self.scale_tensor: Optional[torch.Tensor] = None
+        self.growth_tracker: Optional[torch.Tensor] = None
+        self.inv_scale: Optional[torch.Tensor] = None
+
+    def _ensure(self, dev: torch.device) -> None:
+        """Create the device state on `dev` (on the current stream), as GradScaler does lazily."""
+        if self.scale_tensor is None:
+            self.scale_tensor = torch.full((), self._init_scale, dtype=torch.float32, device=dev)
+            self.growth_tracker = torch.full((), self._init_growth_tracker, dtype=torch.int32,
+                                             device=dev)
+            self._refresh()
+
+    def _refresh(self) -> None:
+        # GradScaler.unscale_'s reciprocal, taken in double
+        self.inv_scale = self.scale_tensor.double().reciprocal().float()
+
+    def scale(self, loss: torch.Tensor) -> torch.Tensor:
+        """`loss` times the current scale: backward through it gives scaled gradients."""
+        if not isinstance(loss, torch.Tensor):
+            raise ValueError("DynamicLossScale.scale takes a Tensor, got %s" % type(loss).__name__)
+        self._ensure(loss.device)
+        return loss * self.scale_tensor.to(device=loss.device, non_blocking=True)
+
+    def _update(self, found_inf: torch.Tensor) -> None:
+        """GradScaler.update: back off after an inf / NaN, grow after growth_interval clean steps;
+        then the next iteration's inverse scale."""
+        torch._amp_update_scale_(self.scale_tensor, self.growth_tracker, found_inf,
+                                 self.growth_factor, self.backoff_factor, self.growth_interval)
+        self._refresh()
+
+    def get_scale(self) -> float:
+        return self._init_scale if self.scale_tensor is None else self.scale_tensor.item()
+
+    def state_dict(self) -> dict:
+        return {"scale": self.get_scale(), "growth_factor": self.growth_factor,
+                "backoff_factor": self.backoff_factor, "growth_interval": self.growth_interval,
+                "_growth_tracker": self._init_growth_tracker if self.growth_tracker is None
+                else self.growth_tracker.item()}
+
+    def load_state_dict(self, state_dict: dict) -> None:
+        if len(state_dict) == 0:
+            raise RuntimeError("The source state dict is empty, possibly because it was saved "
+                               "from a disabled instance of GradScaler.")
+        self._init_scale = float(state_dict["scale"])
+        self.growth_factor = float(state_dict["growth_factor"])
+        self.backoff_factor = float(state_dict["backoff_factor"])
+        self.growth_interval = int(state_dict["growth_interval"])
+        self._init_growth_tracker = int(state_dict["_growth_tracker"])
+        if self.scale_tensor is not None:
+            self.scale_tensor.fill_(self._init_scale)
+            self.growth_tracker.fill_(self._init_growth_tracker)
+            self._refresh()
+
+
+def _check_loss_scale(loss_scale) -> Optional[DynamicLossScale]:
+    if loss_scale is not None and not isinstance(loss_scale, DynamicLossScale):
+        raise TypeError("loss_scale must be a DynamicLossScale or None, got %s"
+                        % type(loss_scale).__name__)
+    return loss_scale
+
+
 class _MasterWeightOptimizer(torch.optim.Optimizer):
     """What the master-weight optimizers share: the parameter checks, fp32 masters, the fp32 restore
     of state_dict, bucket and whole-group stepping with the stream ordering, and the device tables
@@ -108,7 +221,7 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
     _FP32_HINT = ""                                      # the stock optimizer for fp32 parameters
 
     def __init__(self, params, defaults: dict, max_grad_norm: Optional[float] = None,
-                 error_if_nonfinite: bool = False):
+                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
         self._group_of: Dict[int, int] = {}          # id(param) -> index of its param group
         self._slot_of: Dict[int, int] = {}           # id(param) -> position in param-group order
         self._tables: Dict[tuple, tuple] = {}        # launch key -> (rows, device table)
@@ -120,6 +233,10 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         self.max_grad_norm = _check_max_grad_norm(max_grad_norm)
         self.error_if_nonfinite = bool(error_if_nonfinite)
         self.grad_norm: Optional[torch.Tensor] = None   # clipping: the last step's pre-clip norm
+        self.loss_scale = _check_loss_scale(loss_scale)
+        self.found_inf: Optional[torch.Tensor] = None   # loss scaling: the last step's verdict
+        self.step_skipped = False                        # loss scaling: the last step was skipped
+        self._found_inf: Optional[torch.Tensor] = None  # loss scaling: this iteration's verdict
         self.table_uploads = 0
         super().__init__(params, defaults)
 
@@ -156,8 +273,10 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         raise NotImplementedError
 
     def _kernel(self, group: dict, table: torch.Tensor, count: int, chunks: int, dtype: int, arg,
-                stream: torch.cuda.Stream, coef: Optional[torch.Tensor]) -> None:
-        """One launch; with `coef` (the device clip coefficient) the clipped kernel."""
+                stream: torch.cuda.Stream, coef: Optional[torch.Tensor],
+                inv_scale: Optional[torch.Tensor]) -> None:
+        """One launch; with `coef` (the device clip coefficient) the clipped kernel; with
+        `inv_scale` (the device inverse loss scale) the unscaled one, clipped too with `coef`."""
         raise NotImplementedError
 
     def _table(self, key: tuple, rows: List[tuple], dev: torch.device) -> torch.Tensor:
@@ -183,9 +302,11 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                                    % name)
 
     def _launch(self, group: dict, pairs, key: tuple, stream: Optional[torch.cuda.Stream] = None,
-                coef: Optional[torch.Tensor] = None) -> None:
+                coef: Optional[torch.Tensor] = None,
+                inv_scale: Optional[torch.Tensor] = None) -> None:
         """Step [(param, grad)] of one param group with the launches _split gives, on `stream` (which
-        must then be current) or the current stream; with `coef`, clipped."""
+        must then be current) or the current stream; with `coef`, clipped; with `inv_scale`,
+        unscaled."""
         self._check_pairs(pairs)
         stream = stream or torch.cuda.current_stream(pairs[0][0].device)
         for sub, entries, arg in self._split(group, pairs):
@@ -196,7 +317,7 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             table = self._table(key + (sub,), rows, dev)
             with torch.cuda.device(dev):
                 self._kernel(group, table, len(rows), chunks, _DTYPES[entries[0][1].dtype], arg,
-                             stream, coef)
+                             stream, coef, inv_scale)
 
     # ---- clipping --------------------------------------------------------------------------------
     def _norm_buffer(self, dev: torch.device) -> torch.Tensor:
@@ -207,30 +328,74 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             self._present = None
         return self._norms
 
+    def _norm_tables(self, pairs, key: tuple, dev: torch.device):
+        """[(dtype, rows, chunks, device table)] of tok_norm_segment_t for [(param, grad)], one per
+        gradient dtype."""
+        by_dtype: Dict[torch.dtype, list] = {}
+        for p, g in pairs:
+            if g.device != dev:
+                raise ValueError("%s clips or checks gradients on one device; got %s and %s"
+                                 % (type(self).__name__, g.device, dev))
+            by_dtype.setdefault(g.dtype, []).append((g, self._slot_of[id(p)]))
+        out = []
+        for dtype, entries in by_dtype.items():
+            rows, chunks = norm_table(entries)
+            out.append((dtype, rows, chunks, self._table(key + (str(dtype),), rows, dev)))
+        return out
+
     def _launch_norms(self, pairs, key: tuple, norms: torch.Tensor,
                       stream: torch.cuda.Stream) -> None:
         """Enqueue on `stream` (current) the norms of [(param, grad)] into their slots of `norms`: one
-        tok_grad_norms call (two kernels) per gradient dtype."""
-        by_dtype: Dict[torch.dtype, list] = {}
-        for p, g in pairs:
-            if g.device != norms.device:
-                raise ValueError("%s clips gradients on one device; got %s and %s"
-                                 % (type(self).__name__, g.device, norms.device))
-            by_dtype.setdefault(g.dtype, []).append((g, self._slot_of[id(p)]))
-        for dtype, entries in by_dtype.items():
-            rows, chunks = norm_table(entries)
-            table = self._table(key + (str(dtype),), rows, norms.device)
+        tok_grad_norms call (two kernels) per gradient dtype.  With a loss scale, the norms of the
+        unscaled gradients (tok_grad_norms_unscaled), which also set this iteration's found_inf."""
+        scaled = self._scaling(norms.device) if self.loss_scale is not None else None
+        for dtype, rows, chunks, table in self._norm_tables(pairs, key, norms.device):
             # caching-allocator scratch on `stream`: freed back to it after this call
             partials = torch.empty(chunks, dtype=torch.float32, device=norms.device)
             with torch.cuda.device(norms.device):
-                _ffi.check(_ffi.lib().tok_grad_norms(
-                    C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype],
-                    C.c_void_p(partials.data_ptr() if chunks else 0),
-                    C.c_void_p(norms.data_ptr()), C.c_void_p(stream.cuda_stream)))
+                if scaled is None:
+                    _ffi.check(_ffi.lib().tok_grad_norms(
+                        C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype],
+                        C.c_void_p(partials.data_ptr() if chunks else 0),
+                        C.c_void_p(norms.data_ptr()), C.c_void_p(stream.cuda_stream)))
+                else:
+                    _ffi.check(_ffi.lib().tok_grad_norms_unscaled(
+                        C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype],
+                        C.c_void_p(scaled[0].data_ptr()),
+                        C.c_void_p(partials.data_ptr() if chunks else 0),
+                        C.c_void_p(norms.data_ptr()), C.c_void_p(scaled[1].data_ptr()),
+                        C.c_void_p(stream.cuda_stream)))
 
-    def _clip_step(self) -> None:
-        """step() with max_grad_norm: the norms no bucket covered, clip_grad_norm_'s total and
-        coefficient, then every clipped launch — on the current stream, after the bucket streams."""
+    # ---- loss scaling ----------------------------------------------------------------------------
+    def _scaling(self, dev: torch.device) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(inv_scale, found_inf) of this iteration, created on the current stream if missing."""
+        self.loss_scale._ensure(dev)
+        if self._found_inf is None:
+            self._found_inf = torch.zeros((), dtype=torch.float32, device=dev)
+        return self.loss_scale.inv_scale, self._found_inf
+
+    def _launch_check(self, pairs, key: tuple, dev: torch.device,
+                      stream: torch.cuda.Stream) -> None:
+        """Enqueue on `stream` (current) the inf / NaN check of [(param, grad)] into this iteration's
+        found_inf: one tok_grad_nonfinite launch per gradient dtype."""
+        _, found_inf = self._scaling(dev)
+        for dtype, rows, chunks, table in self._norm_tables(pairs, key, dev):
+            with torch.cuda.device(dev):
+                _ffi.check(_ffi.lib().tok_grad_nonfinite(
+                    C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype],
+                    C.c_void_p(found_inf.data_ptr()), C.c_void_p(stream.cuda_stream)))
+
+    def _next_iteration(self, found_inf: torch.Tensor) -> None:
+        """GradScaler.update with this iteration's verdict, then a zeroed found_inf for the next."""
+        self.loss_scale._update(found_inf)
+        self.found_inf = found_inf
+        self._found_inf = torch.zeros((), dtype=torch.float32, device=found_inf.device)
+
+    def _deferred_step(self) -> None:
+        """step() with max_grad_norm or a loss scale, on the current stream after the bucket streams:
+        the norms or inf / NaN checks no bucket covered; with clipping, clip_grad_norm_'s total and
+        coefficient; with a loss scale, GradScaler's host read of found_inf; then every clipped or
+        unscaled launch unless an inf or NaN was found; then the scale's update."""
         pending, self._pending = self._pending, []
         rest = []
         for gi, group in enumerate(self.param_groups):
@@ -242,36 +407,56 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                         if id(p) in self._stepped or p.grad is not None)
         self._stepped.clear()
         self._streams.clear()
+        clip, scaling = self.max_grad_norm is not None, self.loss_scale is not None
+        self.step_skipped = False
         if not present:
-            self.grad_norm = torch.tensor(0.0)   # what clip_grad_norm_ returns without gradients
+            if clip:
+                self.grad_norm = torch.tensor(0.0)   # what clip_grad_norm_ returns without gradients
+            # the scale stays: GradScaler.update refuses to run without any inf check recorded
             return
         pairs = [pg for _, prs in rest for pg in prs]
         self._check_pairs(pairs)
         dev = (pairs[0][0] if pairs else next(iter(pending[0][1].values()))[0][0]).device
         stream = torch.cuda.current_stream(dev)
-        norms = self._norm_buffer(dev)
-        if pairs:
-            self._launch_norms(pairs, ("norm", "group"), norms, stream)
-        if len(present) != norms.numel():
-            # clip_grad_norm_ stacks only the gradients that exist: gather their slots, in order
-            if self._present is None or self._present[0] != present:
-                self._present = (present, torch.tensor(present, dtype=torch.int64).to(dev))
-            norms = norms.index_select(0, self._present[1])
-        # torch.nn.utils.clip_grad_norm_'s own expressions (_get_total_norm, _clip_grads_with_norm_)
-        total = torch.linalg.vector_norm(norms, 2.0)
-        if self.error_if_nonfinite and torch.logical_or(total.isnan(), total.isinf()):
-            raise RuntimeError(
-                f"The total norm of order {2.0} for gradients from "
-                "`parameters` is non-finite, so it cannot be clipped. To disable "
-                "this error and scale the gradients by the non-finite norm anyway, "
-                "set `error_if_nonfinite=False`")
-        coef = torch.clamp(self.max_grad_norm / (total + 1e-6), max=1.0)
-        self.grad_norm = total
-        for index, by_group in pending:
-            for gi, prs in by_group.items():
-                self._launch(self.param_groups[gi], prs, ("clip bucket", index, gi), stream, coef)
-        for gi, prs in rest:
-            self._launch(self.param_groups[gi], prs, ("clip group", gi), stream, coef)
+        inv_scale = found_inf = coef = None
+        if scaling:
+            inv_scale, found_inf = self._scaling(dev)
+        if clip:
+            norms = self._norm_buffer(dev)
+            if pairs:
+                self._launch_norms(pairs, ("norm", "group"), norms, stream)
+            if len(present) != norms.numel():
+                # clip_grad_norm_ stacks only the gradients that exist: gather their slots, in order
+                if self._present is None or self._present[0] != present:
+                    self._present = (present, torch.tensor(present, dtype=torch.int64).to(dev))
+                norms = norms.index_select(0, self._present[1])
+            # torch.nn.utils.clip_grad_norm_'s own expressions (_get_total_norm,
+            # _clip_grads_with_norm_)
+            total = torch.linalg.vector_norm(norms, 2.0)
+            if self.error_if_nonfinite and torch.logical_or(total.isnan(), total.isinf()):
+                if scaling:   # the next iteration starts from a clear verdict
+                    self.found_inf, self._found_inf = found_inf, None
+                raise RuntimeError(
+                    f"The total norm of order {2.0} for gradients from "
+                    "`parameters` is non-finite, so it cannot be clipped. To disable "
+                    "this error and scale the gradients by the non-finite norm anyway, "
+                    "set `error_if_nonfinite=False`")
+            coef = torch.clamp(self.max_grad_norm / (total + 1e-6), max=1.0)
+            self.grad_norm = total
+        elif pairs:
+            self._launch_check(pairs, ("check", "group"), dev, stream)
+        if scaling and found_inf.item():   # GradScaler._maybe_opt_step's host read
+            self.step_skipped = True
+        else:
+            for index, by_group in pending:
+                for gi, prs in by_group.items():
+                    self._launch(self.param_groups[gi], prs, ("clip bucket", index, gi), stream,
+                                 coef, inv_scale)
+            for gi, prs in rest:
+                self._launch(self.param_groups[gi], prs, ("clip group", gi), stream, coef,
+                             inv_scale)
+        if scaling:
+            self._next_iteration(found_inf)
 
     @torch.no_grad()
     def step_bucket(self, params: Iterable[torch.Tensor], grads: Iterable[torch.Tensor], index: int,
@@ -281,8 +466,9 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         exchange.  The next step() orders the current stream after `stream`.
 
         With max_grad_norm, enqueue only the bucket's per-tensor gradient norms there and keep the
-        bucket for step(), which steps it once the global norm exists.  `grads` must then hold the
-        averaged gradients until step()."""
+        bucket for step(), which steps it once the global norm exists.  With a loss scale, likewise
+        enqueue only the bucket's inf / NaN check (or, with max_grad_norm, its unscaled norms, which
+        set the same flag).  `grads` must then hold the averaged gradients until step()."""
         by_group: Dict[int, list] = {}
         for p, g in zip(params, grads):
             gi = self._group_of.get(id(p))
@@ -292,12 +478,15 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             return
         dev = next(iter(by_group.values()))[0][0].device
         stream = stream or torch.cuda.current_stream(dev)
-        if self.max_grad_norm is not None:
+        if self.max_grad_norm is not None or self.loss_scale is not None:
             pairs = [pg for prs in by_group.values() for pg in prs]
             self._check_pairs(pairs)
-            norms = self._norm_buffer(dev)
             with torch.cuda.stream(stream):
-                self._launch_norms(pairs, ("norm", "bucket", index), norms, stream)
+                if self.max_grad_norm is not None:
+                    self._launch_norms(pairs, ("norm", "bucket", index), self._norm_buffer(dev),
+                                       stream)
+                else:
+                    self._launch_check(pairs, ("check", "bucket", index), dev, stream)
             self._pending.append((index, by_group))
             self._stepped.update(id(p) for p, _ in pairs)
             if stream not in self._streams:
@@ -318,8 +507,8 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                 loss = closure()
         for s in self._streams:
             torch.cuda.current_stream(s.device).wait_stream(s)
-        if self.max_grad_norm is not None:
-            self._clip_step()
+        if self.max_grad_norm is not None or self.loss_scale is not None:
+            self._deferred_step()
             return loss
         for gi, group in enumerate(self.param_groups):
             pairs = [(p, p.grad) for p in group["params"]
@@ -338,7 +527,7 @@ class MasterWeightSGD(_MasterWeightOptimizer):
     def __init__(self, params, lr: float, momentum: float = 0.0, dampening: float = 0.0,
                  weight_decay: float = 0.0, nesterov: bool = False, *, maximize: bool = False,
                  differentiable: bool = False, max_grad_norm: Optional[float] = None,
-                 error_if_nonfinite: bool = False):
+                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
         if lr < 0.0:
             raise ValueError("Invalid learning rate: %r" % lr)
         if momentum < 0.0:
@@ -351,7 +540,7 @@ class MasterWeightSGD(_MasterWeightOptimizer):
             raise ValueError("MasterWeightSGD supports neither maximize nor differentiable")
         super().__init__(params, dict(lr=lr, momentum=momentum, dampening=dampening,
                                       weight_decay=weight_decay, nesterov=nesterov),
-                         max_grad_norm, error_if_nonfinite)
+                         max_grad_norm, error_if_nonfinite, loss_scale)
 
     def _split(self, group: dict, pairs) -> List[tuple]:
         """One launch per momentum state: fresh buffers (subkey 1), then the rest (subkey 0)."""
@@ -368,10 +557,14 @@ class MasterWeightSGD(_MasterWeightOptimizer):
             old.append((g, p, st["master_param"], m))
         return [(1, fresh, 1), (0, old, 0)]
 
-    def _kernel(self, group, table, count, chunks, dtype, fresh, stream, coef) -> None:
+    def _kernel(self, group, table, count, chunks, dtype, fresh, stream, coef, inv_scale) -> None:
         args = [C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], group["momentum"],
                 group["dampening"], group["weight_decay"], int(group["nesterov"]), fresh]
-        if coef is None:
+        if inv_scale is not None:
+            _ffi.check(_ffi.lib().tok_sgd_master_step_unscaled(
+                *args, C.c_void_p(inv_scale.data_ptr()),
+                C.c_void_p(0 if coef is None else coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
+        elif coef is None:
             _ffi.check(_ffi.lib().tok_sgd_master_step(*args, C.c_void_p(stream.cuda_stream)))
         else:
             _ffi.check(_ffi.lib().tok_sgd_master_step_clipped(
@@ -389,7 +582,7 @@ class MasterWeightAdam(_MasterWeightOptimizer):
                  foreach: Optional[bool] = None, maximize: bool = False, capturable: bool = False,
                  differentiable: bool = False, fused: Optional[bool] = None,
                  decoupled_weight_decay: bool = False, max_grad_norm: Optional[float] = None,
-                 error_if_nonfinite: bool = False):
+                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
         name = type(self).__name__
         if isinstance(lr, torch.Tensor) or any(isinstance(b, torch.Tensor) for b in betas):
             raise ValueError("%s takes lr and betas as Python floats, not Tensors" % name)
@@ -410,7 +603,7 @@ class MasterWeightAdam(_MasterWeightOptimizer):
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay,
                                       amsgrad=amsgrad,
                                       decoupled_weight_decay=decoupled_weight_decay),
-                         max_grad_norm, error_if_nonfinite)
+                         max_grad_norm, error_if_nonfinite, loss_scale)
 
     def load_state_dict(self, state_dict: dict) -> None:
         super().load_state_dict(state_dict)
@@ -442,12 +635,16 @@ class MasterWeightAdam(_MasterWeightOptimizer):
         ordered = sorted(launches.items(), key=lambda kv: (-kv[0][0], str(kv[0][1])))
         return [(i, entries, step) for i, ((step, _), entries) in enumerate(ordered)]
 
-    def _kernel(self, group, table, count, chunks, dtype, step, stream, coef) -> None:
+    def _kernel(self, group, table, count, chunks, dtype, step, stream, coef, inv_scale) -> None:
         beta1, beta2 = group["betas"]
         args = [C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], beta1, beta2,
                 group["eps"], group["weight_decay"], int(group["decoupled_weight_decay"]),
                 int(group["amsgrad"]), step]
-        if coef is None:
+        if inv_scale is not None:
+            _ffi.check(_ffi.lib().tok_adam_master_step_unscaled(
+                *args, C.c_void_p(inv_scale.data_ptr()),
+                C.c_void_p(0 if coef is None else coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
+        elif coef is None:
             _ffi.check(_ffi.lib().tok_adam_master_step(*args, C.c_void_p(stream.cuda_stream)))
         else:
             _ffi.check(_ffi.lib().tok_adam_master_step_clipped(
@@ -463,8 +660,9 @@ class MasterWeightAdamW(MasterWeightAdam):
                  eps: float = 1e-8, weight_decay: float = 1e-2, amsgrad: bool = False, *,
                  maximize: bool = False, foreach: Optional[bool] = None, capturable: bool = False,
                  differentiable: bool = False, fused: Optional[bool] = None,
-                 max_grad_norm: Optional[float] = None, error_if_nonfinite: bool = False):
+                 max_grad_norm: Optional[float] = None, error_if_nonfinite: bool = False,
+                 loss_scale: Optional[DynamicLossScale] = None):
         super().__init__(params, lr, betas, eps, weight_decay, amsgrad, foreach=foreach,
                          maximize=maximize, capturable=capturable, differentiable=differentiable,
                          fused=fused, decoupled_weight_decay=True, max_grad_norm=max_grad_norm,
-                         error_if_nonfinite=error_if_nonfinite)
+                         error_if_nonfinite=error_if_nonfinite, loss_scale=loss_scale)

@@ -46,7 +46,9 @@ class Replica:
         optimizer (a torch_on_k8s_b200.optim.MasterWeightSGD, MasterWeightAdam or MasterWeightAdamW
         over the model's parameters): the hook steps each bucket's parameters right behind the
         bucket's exchange; optimizer.step() then launches nothing for them.  With max_grad_norm the
-        hook enqueues only the bucket's gradient norms, and optimizer.step() steps every bucket."""
+        hook enqueues only the bucket's gradient norms, and optimizer.step() steps every bucket.
+        With a loss scale the hook enqueues only the bucket's inf / NaN check (or its unscaled
+        norms), and optimizer.step() steps every bucket unless an inf or NaN was found."""
         from torch.nn.parallel import DistributedDataParallel as DDP
         pooled = zero_copy and self.world > 1 and wire_dtype is None
         if pooled:

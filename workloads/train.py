@@ -17,7 +17,8 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 
-def build(name: str):
+def build(name: str, half=None):
+    """(model, input shape, classes, dtype); `half` is resnet50's dtype (default bf16)."""
     import torch
     if name == "mlp":
         from workloads.mlp import mlp
@@ -25,7 +26,7 @@ def build(name: str):
     if name == "resnet50":
         from workloads.resnet50 import resnet50
         torch.manual_seed(0)
-        return resnet50(), (3, 224, 224), 1000, torch.bfloat16
+        return resnet50(), (3, 224, 224), 1000, half or torch.bfloat16
     raise SystemExit("unknown --model %s" % name)
 
 
@@ -44,23 +45,33 @@ def main() -> int:
     ap.add_argument("--clip-grad-norm", type=float, default=None, metavar="X",
                     help="clip the global gradient L2 norm at X: max_grad_norm=X with "
                          "--master-weights, else torch.nn.utils.clip_grad_norm_ before opt.step()")
+    ap.add_argument("--dtype", choices=("bf16", "f16"), default="bf16",
+                    help="the model's dtype (resnet50; f16 takes the stock batch norm)")
+    ap.add_argument("--loss-scale", action="store_true",
+                    help="dynamic loss scaling with torch.amp.GradScaler's defaults "
+                         "(torch_on_k8s_b200.optim.DynamicLossScale); needs --master-weights")
     a = ap.parse_args()
+    if a.loss_scale and not a.master_weights:
+        ap.error("--loss-scale needs --master-weights: stock GradScaler refuses f16 gradients")
 
     import torch
     from torch_on_k8s_b200.sampler import ReplicaSampler
     from torch_on_k8s_b200.worker import init_replica, report_metric
 
     rep = init_replica()
-    model, shape, classes, dtype = build(a.model)
+    model, shape, classes, dtype = build(a.model, {"bf16": torch.bfloat16,
+                                                   "f16": torch.float16}[a.dtype])
     model = model.to(rep.device).to(dtype)
     if len(shape) == 3:
         model = model.to(memory_format=torch.channels_last)
     if a.master_weights:
-        from torch_on_k8s_b200.optim import MasterWeightAdamW, MasterWeightSGD
-        opt = MasterWeightAdamW(model.parameters(), max_grad_norm=a.clip_grad_norm) \
+        from torch_on_k8s_b200.optim import DynamicLossScale, MasterWeightAdamW, MasterWeightSGD
+        ls = DynamicLossScale() if a.loss_scale else None
+        opt = MasterWeightAdamW(model.parameters(), max_grad_norm=a.clip_grad_norm,
+                                loss_scale=ls) \
             if a.optimizer == "adamw" else \
             MasterWeightSGD(model.parameters(), lr=0.01, momentum=0.9,
-                            max_grad_norm=a.clip_grad_norm)
+                            max_grad_norm=a.clip_grad_norm, loss_scale=ls)
         ddp, hook = rep.wrap(model, record_events=(rep.rank == 0), optimizer=opt)
     else:
         ddp, hook = rep.wrap(model, record_events=(rep.rank == 0))
@@ -77,7 +88,7 @@ def main() -> int:
         opt.zero_grad(set_to_none=True)
         out = ddp(x).float()
         loss = torch.nn.functional.cross_entropy(out, y)
-        loss.backward()
+        (opt.loss_scale.scale(loss) if a.loss_scale else loss).backward()
         grad_norm = None
         if a.clip_grad_norm is not None and not a.master_weights:
             # after backward: DDP's hook has averaged the gradients by now
@@ -94,7 +105,10 @@ def main() -> int:
             print("Epoch: [0][%4d/%d]\tTime %6.3f (%6.3f)\tData  0.000 ( 0.000)\tLoss %.4e\t"
                   "Acc@1 %6.2f (%6.2f)\tAcc@5 %6.2f (%6.2f)" %
                   (step + 1, a.steps, lat, lat, float(loss), acc, acc, acc, acc) +
-                  ("" if grad_norm is None else "\tGradNorm %.4e" % float(grad_norm)), flush=True)
+                  ("" if grad_norm is None else "\tGradNorm %.4e" % float(grad_norm)) +
+                  ("\tScale %.1f%s" % (opt.loss_scale.get_scale(),
+                                       " (skipped)" if opt.step_skipped else "")
+                   if a.loss_scale else ""), flush=True)
             if rep.rank == 0 and rep.world > 1:
                 ev = hook.drain_events()       # [(wire bytes, bucket bytes, exchange ms, wait ms)]
                 ms = sum(e[2] for e in ev)

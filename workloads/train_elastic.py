@@ -25,8 +25,11 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 
-def build(name: str, batch: int, rank: int, dev):
+def build(name: str, batch: int, rank: int, dev, half=None):
+    """(model, loss of the wrapped model, work units per step); `half` is the dtype of bert and
+    resnet50 (default bf16)."""
     import torch
+    half = half or torch.bfloat16
     if name == "mlp":
         from workloads.mlp import batch as mk, mlp
         model = mlp(0).to(dev)
@@ -35,15 +38,15 @@ def build(name: str, batch: int, rank: int, dev):
         return model, (lambda m: torch.nn.functional.cross_entropy(m(x), y)), batch
     if name == "bert":
         from workloads.bert import batch as mk, bert_base, loss_fn
-        model = bert_base().to(dev).to(torch.bfloat16)
+        model = bert_base().to(dev).to(half)
         ids = mk(rank, batch).to(dev)
         return model, (lambda m: loss_fn(m, ids)), batch * ids.shape[1]
     if name == "resnet50":
         from workloads.resnet50 import resnet50
         torch.manual_seed(0)
-        model = resnet50().to(dev).to(torch.bfloat16).to(memory_format=torch.channels_last)
+        model = resnet50().to(dev).to(half).to(memory_format=torch.channels_last)
         gen = torch.Generator().manual_seed(1234 + rank)
-        x = torch.randn(batch, 3, 224, 224, generator=gen).to(torch.bfloat16).to(dev) \
+        x = torch.randn(batch, 3, 224, 224, generator=gen).to(half).to(dev) \
             .contiguous(memory_format=torch.channels_last)
         y = torch.randint(0, 1000, (batch,), generator=gen).to(dev)
         return model, (lambda m: torch.nn.functional.cross_entropy(m(x).float(), y)), batch
@@ -67,7 +70,15 @@ def main() -> int:
                     help="clip the global gradient L2 norm at X: max_grad_norm=X with "
                          "--master-weights, else torch.nn.utils.clip_grad_norm_ between the "
                          "exchange and opt.step()")
+    ap.add_argument("--dtype", choices=("bf16", "f16"), default="bf16",
+                    help="the model's dtype (bert, resnet50; resnet50 in f16 takes the stock "
+                         "batch norm)")
+    ap.add_argument("--loss-scale", action="store_true",
+                    help="dynamic loss scaling with torch.amp.GradScaler's defaults "
+                         "(torch_on_k8s_b200.optim.DynamicLossScale); needs --master-weights")
     a = ap.parse_args()
+    if a.loss_scale and not a.master_weights:
+        ap.error("--loss-scale needs --master-weights: stock GradScaler refuses f16 gradients")
 
     t_proc = time.time()
     import torch
@@ -81,17 +92,20 @@ def main() -> int:
     torch.cuda.set_device(gpu)
     dev = torch.device("cuda", gpu)
     data_rank = int(os.environ.get("RANK", "0"))
-    model, loss_of, units = build(a.model, a.batch, data_rank, dev)
+    model, loss_of, units = build(a.model, a.batch, data_rank, dev,
+                                  {"bf16": torch.bfloat16, "f16": torch.float16}[a.dtype])
     rep = init_replica(bootstrap_backend=None, device=gpu)   # no torch.distributed: the world may change
     joined_at_epoch = rep.comm.caps().epoch
     name = os.environ.get("TOK8S_REPLICA", "replica-%d" % rep.rank)
     edp = ElasticDataParallel(model, rep.comm, bucket_cap_mb=25)
     if a.master_weights:
-        from torch_on_k8s_b200.optim import MasterWeightAdamW, MasterWeightSGD
-        opt = MasterWeightAdamW(model.parameters(), lr=a.lr, max_grad_norm=a.clip_grad_norm) \
+        from torch_on_k8s_b200.optim import DynamicLossScale, MasterWeightAdamW, MasterWeightSGD
+        ls = DynamicLossScale() if a.loss_scale else None
+        opt = MasterWeightAdamW(model.parameters(), lr=a.lr, max_grad_norm=a.clip_grad_norm,
+                                loss_scale=ls) \
             if a.optimizer == "adamw" else \
             MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9,
-                            max_grad_norm=a.clip_grad_norm)
+                            max_grad_norm=a.clip_grad_norm, loss_scale=ls)
     else:
         opt = torch.optim.AdamW(model.parameters(), lr=a.lr) if a.optimizer == "adamw" else \
             torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
@@ -133,7 +147,7 @@ def main() -> int:
             t_prev = time.time()
         edp.zero_grad()
         loss = loss_of(edp)
-        loss.backward()
+        (opt.loss_scale.scale(loss) if a.loss_scale else loss).backward()
         edp.reduce_grads(optimizer=opt if a.master_weights else None)
         grad_norm = None
         if a.clip_grad_norm is not None and not a.master_weights:
@@ -147,7 +161,9 @@ def main() -> int:
         step += 1
         lat_acc.append(dt)
         log(event="step", step=step, seconds=dt, units=units, loss=float(loss),
-            **({} if grad_norm is None else dict(grad_norm=float(grad_norm))))
+            **({} if grad_norm is None else dict(grad_norm=float(grad_norm))),
+            **(dict(scale=opt.loss_scale.get_scale(), skipped=opt.step_skipped)
+               if a.loss_scale else {}))
         if step % a.log_every == 0 and rep.rank <= 1:
             lat = sum(lat_acc) / len(lat_acc)
             lat_acc = []
