@@ -380,6 +380,42 @@ int tok_grad_norms_unscaled(const tok_norm_segment_t* segments, int count, int64
 int tok_grad_nonfinite(const tok_norm_segment_t* segments, int count, int64_t chunks, int dtype,
                        float* found_inf, void* cuda_stream);
 
+/* LAMB step on fp32 master weights for bf16 / f16 parameters (torch_on_k8s_b200/optim.py's
+ * MasterWeightLAMB), apex FusedLAMB's algorithm in its defaults (adam_w_mode, bias correction, no
+ * trust ratio where weight_decay == 0), for the parameters of one param group that share a step count.
+ * For every segment it produces the bits of the torch loop on the fp32 masters W, with M exp_avg, V
+ * exp_avg_sq and G = f32(grad):
+ *   _foreach_lerp_(M, G, 1 - beta1); _foreach_mul_(V, beta2); _foreach_addcmul_(V, G, G, 1 - beta2)
+ *   D = _foreach_sqrt(V) / bc2_sqrt + eps;  U = M / bc1 / D;  U += weight_decay * W   (wd != 0)
+ *   c = lr * (|W| > 0 and |U| > 0 ? |W| / |U| : 1)  (wd != 0, norms of _foreach_norm)  else  c = lr
+ *   W = W - U * c   (two roundings);  param.copy_(W)                                     (RNE)
+ * with bc1 = 1 - beta1^step and bc2_sqrt = (1 - beta2^step)^0.5 computed in double from `step`, the
+ * parameters' step count after its increment (>= 1).  With `inv_scale` not NULL, G = f32(grad) *
+ * *inv_scale (one rounding); with `grad_coef` not NULL, G = G * *grad_coef follows (one more rounding):
+ * tok_adam_master_step_unscaled's gradient.  Both are DEVICE fp32 scalars.
+ * The table follows tok_grad_norms's rules (TOK_NORM_CHUNK elements per chunk, one CTA per chunk, a
+ * DEVICE array): each norm keeps _foreach_norm's chunking and reduction trees.  `partials` is DEVICE
+ * fp32 scratch of 2 * `chunks` elements (written only when weight_decay != 0).  Two launches, none
+ * when `chunks` is 0: the first updates M and V and writes each chunk's partial sums of W^2 and U^2;
+ * the second reduces a segment's partials in each of its CTAs and updates W and param.  Returns
+ * TOK_ERR_INVALID for a null or empty table, a negative or too large `chunks`, a dtype other than
+ * TOK_BF16 / TOK_F16, a negative or non-finite lr, eps or weight_decay, betas outside [0, 1), a step
+ * below 1 or non-finite, null partials with chunks, TOK_ERR_NO_DEVICE without a GPU.  Enqueued on
+ * `cuda_stream`, no synchronisation. */
+typedef struct tok_lamb_segment {
+  const void* grad;   /* bf16 / f16[numel], the parameter's gradient (anywhere in its bucket)     */
+  void* param;        /* bf16 / f16[numel], written                                               */
+  float* master;      /* fp32[numel], dense, read and written                                     */
+  float* exp_avg;     /* fp32[numel], dense, read and written                                     */
+  float* exp_avg_sq;  /* fp32[numel], dense, read and written                                     */
+  int64_t numel;
+  int64_t chunk0;     /* index of this segment's first chunk, counted in TOK_NORM_CHUNKs          */
+} tok_lamb_segment_t;
+int tok_lamb_master_step(const tok_lamb_segment_t* segments, int count, int64_t chunks, int dtype,
+                         double lr, double beta1, double beta2, double eps, double weight_decay,
+                         double step, float* partials, const float* inv_scale,
+                         const float* grad_coef, void* cuda_stream);
+
 /* Which algorithm AUTO picks for `wire_bytes` on this communicator. */
 int tok_allreduce_algo(tok_comm_t* comm, size_t wire_bytes, int* algo);
 /* Number of kernels this communicator has launched so far (bench.py's gpu_launches): exchange,

@@ -43,12 +43,12 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "norm_reduce.h"
 #include "tok_internal.h"
 
 namespace tok {
 namespace {
 
-constexpr int kNormThreads = 512;              // ATen's kBlockSize, and lpnorm_cleanup's block
 constexpr int64_t kNormChunk = TOK_NORM_CHUNK;  // ATen's kChunkSize for multi_tensor_apply
 constexpr int kIlp = 4;                        // ATen's kILP
 constexpr int kAhead = 8;                      // float4 groups loaded before their FMAs run
@@ -60,23 +60,6 @@ template <> __device__ __forceinline__ float to_f32<__nv_bfloat16>(uint16_t bits
 }
 template <> __device__ __forceinline__ float to_f32<__half>(uint16_t bits) {
   return __half2float(__ushort_as_half(bits));
-}
-
-// ATen's BlockReduceSum for a 512-thread block; the sum is valid in thread 0.
-__device__ __forceinline__ float block_sum(float val, float* shared) {
-  const int lid = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) val = __fadd_rn(val, __shfl_down_sync(0xffffffffu, val, off));
-  __syncthreads();
-  if (lid == 0) shared[wid] = val;
-  __syncthreads();
-  val = threadIdx.x < kNormThreads / 32 ? shared[lid] : 0.0f;
-  if (wid == 0) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1)
-      val = __fadd_rn(val, __shfl_down_sync(0xffffffffu, val, off));
-  }
-  return val;
 }
 
 // The exponent bits of T: a value is inf or NaN when all of them are set.
@@ -202,11 +185,7 @@ __global__ void __launch_bounds__(kNormThreads)
                        const float* __restrict__ partials, float* __restrict__ norms) {
   __shared__ float red[32];
   const tok_norm_segment_t s = seg[blockIdx.x];
-  const int64_t nchunks = (s.numel + kNormChunk - 1) / kNormChunk;
-  float val = 0.0f;
-  for (int64_t i = threadIdx.x; i < nchunks; i += kNormThreads)
-    val = __fadd_rn(val, partials[s.chunk0 + i]);
-  val = block_sum(val, red);
+  const float val = cleanup_sum(partials + s.chunk0, (s.numel + kNormChunk - 1) / kNormChunk, red);
   if (threadIdx.x == 0) norms[s.slot] = __fsqrt_rn(val);
 }
 

@@ -71,6 +71,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "master_elem.h"
 #include "tok_internal.h"
 
 namespace tok {
@@ -82,22 +83,6 @@ static_assert(kChunk % 8 == 0, "a chunk must start at a vector boundary of every
 
 __device__ __forceinline__ float add_alpha(float a, float b, float alpha) {
   return __fmaf_rn(alpha, b, a);   // a + alpha * b, one rounding (see the header comment)
-}
-
-template <typename T> __device__ __forceinline__ float widen(uint16_t bits);
-template <> __device__ __forceinline__ float widen<__nv_bfloat16>(uint16_t bits) {
-  return __uint_as_float((uint32_t)bits << 16);
-}
-template <> __device__ __forceinline__ float widen<__half>(uint16_t bits) {
-  return __half2float(__ushort_as_half(bits));
-}
-
-template <typename T> __device__ __forceinline__ uint16_t narrow(float v);
-template <> __device__ __forceinline__ uint16_t narrow<__nv_bfloat16>(float v) {
-  return __bfloat16_as_ushort(__float2bfloat16_rn(v));   // what c10::BFloat16(float) does on sm_80+
-}
-template <> __device__ __forceinline__ uint16_t narrow<__half>(float v) {
-  return __half_as_ushort(__float2half_rn(v));
 }
 
 __device__ __forceinline__ float lane(const float4& v, int k) {
@@ -128,16 +113,6 @@ __device__ __forceinline__ void store_param8(void* param, int64_t i, const uint1
   *(uint4*)((uint16_t*)param + i) =
       make_uint4(out[0] | ((uint32_t)out[1] << 16), out[2] | ((uint32_t)out[3] << 16),
                  out[4] | ((uint32_t)out[5] << 16), out[6] | ((uint32_t)out[7] << 16));
-}
-
-// The gradient element as the optimizer reads it: f32(grad); with kUnscale that times the inverse loss
-// scale, rounded once, as GradScaler.unscale_ stores master.grad; with kClip that times the clip
-// coefficient, rounded once, as torch's clip_grad_norm_ multiplies master.grad (_foreach_mul_) before
-// the optimizer step reads it.
-template <typename T, bool kClip, bool kUnscale>
-__device__ __forceinline__ float grad_in(uint16_t bits, float coef, float inv_scale) {
-  const float g = kUnscale ? __fmul_rn(widen<T>(bits), inv_scale) : widen<T>(bits);
-  return kClip ? __fmul_rn(g, coef) : g;
 }
 
 // Chunk blockIdx.x of the table in `a` (a Step: SgdArgs or AdamArgs).  Thread 0 finds the last entry
@@ -281,12 +256,6 @@ __global__ void __launch_bounds__(kSgdThreads)
 }
 
 // ---- Adam / AdamW -------------------------------------------------------------------------------
-// at::native::lerp: |w| < 0.5 ? m + w*(g-m) : g - (g-m)*(1-w), each branch one FMA (the probe).
-__device__ __forceinline__ float lerp(float m, float g, float w) {
-  const float d = __fsub_rn(g, m);
-  return fabsf(w) < 0.5f ? __fmaf_rn(w, d, m) : __fmaf_rn(-d, __fsub_rn(1.0f, w), g);
-}
-
 struct AdamArgs {
   using Segment = tok_adam_segment_t;
   const tok_adam_segment_t* seg;
@@ -311,8 +280,7 @@ struct AdamArgs {
       else g = add_alpha(g, w, wd);
     }
     m = lerp(m, g, lerp_w);
-    v = __fmul_rn(v, beta2);
-    v = sq_value == 1.0f ? __fmaf_rn(g, g, v) : __fmaf_rn(sq_value, __fmul_rn(g, g), v);
+    v = second_moment(v, g, beta2, sq_value);
     float d = v;
     if (amsgrad) d = vmax = (isnan(vmax) || vmax > v) ? vmax : v;   // ATen's maximum
     d = __fadd_rn(__fdiv_rn(__fsqrt_rn(d), bc2_sqrt), eps);

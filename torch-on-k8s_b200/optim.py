@@ -1,5 +1,5 @@
-"""SGD, Adam and AdamW on fp32 master weights for bf16 / f16 models, stepped by one libtok8s kernel per
-bucket.
+"""SGD, Adam, AdamW and LAMB on fp32 master weights for bf16 / f16 models, stepped by libtok8s kernels
+per bucket.
 
 bf16 keeps 8 significant bits: `torch.optim.SGD` on bf16 parameters rounds away every update smaller
 than about 1/256 of the weight, and an Adam update is at most about `lr`.  These optimizers keep, per
@@ -13,7 +13,35 @@ under torch's keys, and one step produces the bits of
 
 in a single pass over gradient, master, optimizer state and parameter (csrc/optim.cu).
 MasterWeightSGD keeps `momentum_buffer`; MasterWeightAdam and MasterWeightAdamW keep `exp_avg`,
-`exp_avg_sq`, `max_exp_avg_sq` (amsgrad) and a CPU float32 `step`, as torch does.
+`exp_avg_sq`, `max_exp_avg_sq` (amsgrad) and a CPU float32 `step`, as torch does; MasterWeightLAMB
+keeps the same keys but `max_exp_avg_sq`.
+
+MasterWeightLAMB is LAMB (You et al., 2019) as apex FusedLAMB runs it in its defaults (adam_w_mode,
+bias_correction, grad_averaging, use_nvlamb=False).  torch has no LAMB, so this is the restatement it
+matches bit for bit, per param group, on the masters W with M exp_avg, V exp_avg_sq and G the fp32
+master.grad (f32(grad), times the inverse loss scale, times the clip coefficient, as below):
+
+    torch._foreach_lerp_(M, G, 1 - beta1)
+    torch._foreach_mul_(V, beta2)
+    torch._foreach_addcmul_(V, G, G, 1 - beta2)
+    D = torch._foreach_sqrt(V); torch._foreach_div_(D, bc2_sqrts); torch._foreach_add_(D, eps)
+    U = torch._foreach_div(M, bc1s); torch._foreach_div_(U, D)
+    if weight_decay != 0:                         # decided on the Python float, per group
+        torch._foreach_add_(U, W, alpha=weight_decay)
+        wn, un = torch._foreach_norm(W), torch._foreach_norm(U)   # W before this step's update
+        C = [torch.where((a > 0) & (b > 0), a / b, 1.0) * lr for a, b in zip(wn, un)]
+    else:
+        C = [lr] * len(W)                         # no trust ratio: apex FusedLAMB's default
+    for w, u, c in zip(W, U, C):
+        w.sub_(u * c)                             # two roundings: u*c, then w - (u*c)
+    P.copy_(W)                                    # round to nearest even into bf16 / f16
+
+with bc1s[i] = 1 - beta1 ** step_i and bc2_sqrts[i] = (1 - beta2 ** step_i) ** 0.5 from each
+parameter's own step count, in Python doubles, as torch's Adam computes them.  Two kernels per launch
+(csrc/lamb.cu): the moments and the chunk partials of both norms, then the trust ratio and the update.
+Unlike apex, clipping is clip_grad_norm_'s max_grad_norm= below, and the defaults are lr=1e-3,
+betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01.  The trust ratio is per parameter, so a bucket's full
+LAMB step runs behind its own exchange, as Adam's does.
 
 Used on its own, step() steps every parameter that has a gradient.  Handed to
 `Replica.wrap(..., optimizer=opt)` or `ElasticDataParallel.reduce_grads(optimizer=opt)`, the step of
@@ -90,16 +118,16 @@ def _dense(t: torch.Tensor) -> bool:
     return True
 
 
-def segment_table(entries) -> Tuple[List[tuple], int]:
-    """Rows of tok_sgd_segment_t / tok_adam_segment_t — (grad, param, *fp32 state, numel, chunk0) as
-    integers, 0 for a None state tensor — for [(grad, param, *fp32 state)], and the total number of
-    chunks."""
+def segment_table(entries, chunk: int = CHUNK) -> Tuple[List[tuple], int]:
+    """Rows of tok_sgd_segment_t / tok_adam_segment_t / tok_lamb_segment_t — (grad, param, *fp32
+    state, numel, chunk0) as integers, 0 for a None state tensor — for [(grad, param, *fp32 state)],
+    and the total number of chunks of `chunk` elements (NORM_CHUNK for LAMB)."""
     rows, chunks = [], 0
     for g, p, *state in entries:
         n = p.numel()
         rows.append((g.data_ptr(), p.data_ptr(), *(0 if t is None else t.data_ptr() for t in state),
                      n, chunks))
-        chunks += -(-n // CHUNK)
+        chunks += -(-n // chunk)
     return rows, chunks
 
 
@@ -219,6 +247,7 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
 
     _FP32_STATE: Tuple[str, ...] = ("master_param",)   # state restored to fp32 by load_state_dict
     _FP32_HINT = ""                                      # the stock optimizer for fp32 parameters
+    _CHUNK = CHUNK                                       # elements per chunk of the step's table
 
     def __init__(self, params, defaults: dict, max_grad_norm: Optional[float] = None,
                  error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
@@ -313,7 +342,7 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             if not entries:
                 continue
             dev = entries[0][1].device
-            rows, chunks = segment_table(entries)
+            rows, chunks = segment_table(entries, self._CHUNK)
             table = self._table(key + (sub,), rows, dev)
             with torch.cuda.device(dev):
                 self._kernel(group, table, len(rows), chunks, _DTYPES[entries[0][1].dtype], arg,
@@ -520,6 +549,38 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         return loss
 
 
+def _own_cpu_steps(opt: _MasterWeightOptimizer, state_dict: dict) -> None:
+    """After load_state_dict: a CPU float32 step of the optimizer's own, not the saved tensor, since
+    step() counts in place."""
+    params = [p for g in opt.param_groups for p in g["params"]]
+    for i, saved in state_dict["state"].items():
+        if "step" in saved:
+            opt.state[params[i]]["step"] = torch.as_tensor(saved["step"]).to(
+                "cpu", torch.float32, copy=True)
+
+
+def _split_by_step(opt: _MasterWeightOptimizer, pairs, amsgrad: bool) -> List[tuple]:
+    """Adam's and LAMB's _split: create missing state as torch's first Adam step does, count the step,
+    and launch once per (step count, dtype) — normally one launch.  A parameter skipped for lack of a
+    gradient falls behind and gets its own launch, as torch's bias corrections are per parameter.
+    Entries are (grad, param, master, exp_avg, exp_avg_sq, max_exp_avg_sq or None)."""
+    launches: Dict[tuple, list] = {}
+    for p, g in pairs:
+        st = opt.state[p]
+        w = st["master_param"]
+        if "step" not in st:
+            st["step"] = torch.tensor(0.0, dtype=torch.float32)
+            st["exp_avg"] = torch.zeros_like(w, memory_format=torch.preserve_format)
+            st["exp_avg_sq"] = torch.zeros_like(w, memory_format=torch.preserve_format)
+        if amsgrad and "max_exp_avg_sq" not in st:
+            st["max_exp_avg_sq"] = torch.zeros_like(w, memory_format=torch.preserve_format)
+        st["step"] += 1
+        launches.setdefault((st["step"].item(), p.dtype), []).append(
+            (g, p, w, st["exp_avg"], st["exp_avg_sq"], st["max_exp_avg_sq"] if amsgrad else None))
+    ordered = sorted(launches.items(), key=lambda kv: (-kv[0][0], str(kv[0][1])))
+    return [(i, entries, step) for i, ((step, _), entries) in enumerate(ordered)]
+
+
 class MasterWeightSGD(_MasterWeightOptimizer):
     _FP32_STATE = ("master_param", "momentum_buffer")
     _FP32_HINT = "torch.optim.SGD(fused=True)"
@@ -607,33 +668,10 @@ class MasterWeightAdam(_MasterWeightOptimizer):
 
     def load_state_dict(self, state_dict: dict) -> None:
         super().load_state_dict(state_dict)
-        # a CPU float32 step of this optimizer's own, not the saved tensor: step() counts in place
-        params = [p for g in self.param_groups for p in g["params"]]
-        for i, saved in state_dict["state"].items():
-            if "step" in saved:
-                self.state[params[i]]["step"] = torch.as_tensor(saved["step"]).to(
-                    "cpu", torch.float32, copy=True)
+        _own_cpu_steps(self, state_dict)
 
     def _split(self, group: dict, pairs) -> List[tuple]:
-        """Create missing state as torch's first step does, count the step, and launch once per
-        (step count, dtype) — normally one launch.  A parameter skipped for lack of a gradient falls
-        behind and gets its own launch, as torch's bias corrections are per parameter."""
-        launches: Dict[tuple, list] = {}
-        for p, g in pairs:
-            st = self.state[p]
-            w = st["master_param"]
-            if "step" not in st:
-                st["step"] = torch.tensor(0.0, dtype=torch.float32)
-                st["exp_avg"] = torch.zeros_like(w, memory_format=torch.preserve_format)
-                st["exp_avg_sq"] = torch.zeros_like(w, memory_format=torch.preserve_format)
-            if group["amsgrad"] and "max_exp_avg_sq" not in st:
-                st["max_exp_avg_sq"] = torch.zeros_like(w, memory_format=torch.preserve_format)
-            st["step"] += 1
-            launches.setdefault((st["step"].item(), p.dtype), []).append(
-                (g, p, w, st["exp_avg"], st["exp_avg_sq"],
-                 st["max_exp_avg_sq"] if group["amsgrad"] else None))
-        ordered = sorted(launches.items(), key=lambda kv: (-kv[0][0], str(kv[0][1])))
-        return [(i, entries, step) for i, ((step, _), entries) in enumerate(ordered)]
+        return _split_by_step(self, pairs, group["amsgrad"])
 
     def _kernel(self, group, table, count, chunks, dtype, step, stream, coef, inv_scale) -> None:
         beta1, beta2 = group["betas"]
@@ -666,3 +704,66 @@ class MasterWeightAdamW(MasterWeightAdam):
                          maximize=maximize, capturable=capturable, differentiable=differentiable,
                          fused=fused, decoupled_weight_decay=True, max_grad_norm=max_grad_norm,
                          error_if_nonfinite=error_if_nonfinite, loss_scale=loss_scale)
+
+
+class MasterWeightLAMB(_MasterWeightOptimizer):
+    """LAMB (You et al., 2019) on fp32 masters: apex FusedLAMB's algorithm in its defaults, restated
+    with torch ops in the module docstring.  It keeps MasterWeightAdam's state keys.  Each bucket (or
+    param group) takes its full step behind its own exchange: the trust ratio needs the norms of one
+    parameter's master and update, not a global norm."""
+
+    _FP32_STATE = ("master_param", "exp_avg", "exp_avg_sq")
+    _FP32_HINT = "torch.optim has no LAMB to use instead"
+    _CHUNK = NORM_CHUNK   # _foreach_norm's chunks: the trust ratio's norms keep its reduction
+
+    def __init__(self, params, lr: float = 1e-3, betas: Tuple[float, float] = (0.9, 0.999),
+                 eps: float = 1e-6, weight_decay: float = 1e-2, amsgrad: bool = False, *,
+                 maximize: bool = False, capturable: bool = False, differentiable: bool = False,
+                 fused: Optional[bool] = None, max_grad_norm: Optional[float] = None,
+                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
+        name = type(self).__name__
+        if isinstance(lr, torch.Tensor) or any(isinstance(b, torch.Tensor) for b in betas):
+            raise ValueError("%s takes lr and betas as Python floats, not Tensors" % name)
+        if amsgrad or maximize or capturable or differentiable or fused:
+            raise ValueError("%s supports none of amsgrad, maximize, capturable, differentiable and "
+                             "fused" % name)
+        # torch.optim.Adam's checks and messages
+        if not 0.0 <= lr:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if not 0.0 <= eps:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if not 0.0 <= betas[0] < 1.0:
+            raise ValueError(f"Invalid beta parameter at index 0: {betas[0]}")
+        if not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameter at index 1: {betas[1]}")
+        if not 0.0 <= weight_decay:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay),
+                         max_grad_norm, error_if_nonfinite, loss_scale)
+
+    def load_state_dict(self, state_dict: dict) -> None:
+        super().load_state_dict(state_dict)
+        _own_cpu_steps(self, state_dict)
+
+    def _split(self, group: dict, pairs) -> List[tuple]:
+        """Adam's: one launch per (step count, dtype), entries without max_exp_avg_sq."""
+        return [(i, [e[:5] for e in entries], step)
+                for i, entries, step in _split_by_step(self, pairs, False)]
+
+    def _kernel(self, group, table, count, chunks, dtype, step, stream, coef, inv_scale) -> None:
+        beta1, beta2 = group["betas"]
+        # caching-allocator scratch on `stream` (current): the two norm partials of every chunk
+        partials = torch.empty(2 * chunks, dtype=torch.float32, device=table.device)
+        _ffi.check(_ffi.lib().tok_lamb_master_step(
+            C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], beta1, beta2,
+            group["eps"], group["weight_decay"], step, C.c_void_p(partials.data_ptr()),
+            C.c_void_p(0 if inv_scale is None else inv_scale.data_ptr()),
+            C.c_void_p(0 if coef is None else coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
+
+
+def lamb_param_groups(params: Iterable[torch.Tensor], weight_decay: float = 1e-2) -> List[dict]:
+    """BERT's two LAMB param groups: `weight_decay` for the matrices and convolution kernels, none for
+    the 1-D parameters (biases, LayerNorm and BatchNorm weights)."""
+    params = list(params)
+    return [dict(params=[p for p in params if p.dim() > 1], weight_decay=weight_decay),
+            dict(params=[p for p in params if p.dim() <= 1], weight_decay=0.0)]

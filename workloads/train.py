@@ -39,9 +39,11 @@ def main() -> int:
     ap.add_argument("--master-weights", action="store_true",
                     help="bf16 / f16 models: SGD on fp32 master weights, stepped behind each "
                          "bucket's exchange (torch_on_k8s_b200.optim.MasterWeightSGD, or "
-                         "MasterWeightAdamW with --optimizer adamw)")
-    ap.add_argument("--optimizer", choices=("sgd", "adamw"), default="sgd",
-                    help="sgd: lr 0.01, momentum 0.9; adamw: torch.optim.AdamW's defaults")
+                         "MasterWeightAdamW / MasterWeightLAMB with --optimizer adamw / lamb)")
+    ap.add_argument("--optimizer", choices=("sgd", "adamw", "lamb"), default="sgd",
+                    help="sgd: lr 0.01, momentum 0.9; adamw: torch.optim.AdamW's defaults; lamb: "
+                         "MasterWeightLAMB's defaults, no weight decay on 1-D parameters (needs "
+                         "--master-weights)")
     ap.add_argument("--clip-grad-norm", type=float, default=None, metavar="X",
                     help="clip the global gradient L2 norm at X: max_grad_norm=X with "
                          "--master-weights, else torch.nn.utils.clip_grad_norm_ before opt.step()")
@@ -53,6 +55,8 @@ def main() -> int:
     a = ap.parse_args()
     if a.loss_scale and not a.master_weights:
         ap.error("--loss-scale needs --master-weights: stock GradScaler refuses f16 gradients")
+    if a.optimizer == "lamb" and not a.master_weights:
+        ap.error("--optimizer lamb needs --master-weights: torch.optim has no LAMB")
 
     import torch
     from torch_on_k8s_b200.sampler import ReplicaSampler
@@ -65,13 +69,18 @@ def main() -> int:
     if len(shape) == 3:
         model = model.to(memory_format=torch.channels_last)
     if a.master_weights:
-        from torch_on_k8s_b200.optim import DynamicLossScale, MasterWeightAdamW, MasterWeightSGD
+        from torch_on_k8s_b200.optim import (DynamicLossScale, MasterWeightAdamW, MasterWeightLAMB,
+                                             MasterWeightSGD, lamb_param_groups)
         ls = DynamicLossScale() if a.loss_scale else None
-        opt = MasterWeightAdamW(model.parameters(), max_grad_norm=a.clip_grad_norm,
-                                loss_scale=ls) \
-            if a.optimizer == "adamw" else \
-            MasterWeightSGD(model.parameters(), lr=0.01, momentum=0.9,
-                            max_grad_norm=a.clip_grad_norm, loss_scale=ls)
+        if a.optimizer == "lamb":
+            opt = MasterWeightLAMB(lamb_param_groups(model.parameters()),
+                                   max_grad_norm=a.clip_grad_norm, loss_scale=ls)
+        elif a.optimizer == "adamw":
+            opt = MasterWeightAdamW(model.parameters(), max_grad_norm=a.clip_grad_norm,
+                                    loss_scale=ls)
+        else:
+            opt = MasterWeightSGD(model.parameters(), lr=0.01, momentum=0.9,
+                                  max_grad_norm=a.clip_grad_norm, loss_scale=ls)
         ddp, hook = rep.wrap(model, record_events=(rep.rank == 0), optimizer=opt)
     else:
         ddp, hook = rep.wrap(model, record_events=(rep.rank == 0))

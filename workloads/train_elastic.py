@@ -62,10 +62,12 @@ def main() -> int:
     ap.add_argument("--log-every", type=int, default=5)
     ap.add_argument("--master-weights", action="store_true",
                     help="bf16 models: SGD on fp32 master weights, stepped behind each bucket's "
-                         "exchange (torch_on_k8s_b200.optim.MasterWeightSGD, or MasterWeightAdamW "
-                         "with --optimizer adamw)")
-    ap.add_argument("--optimizer", choices=("sgd", "adamw"), default="sgd",
-                    help="sgd: momentum 0.9; adamw: torch.optim.AdamW's defaults but --lr")
+                         "exchange (torch_on_k8s_b200.optim.MasterWeightSGD, or MasterWeightAdamW / "
+                         "MasterWeightLAMB with --optimizer adamw / lamb)")
+    ap.add_argument("--optimizer", choices=("sgd", "adamw", "lamb"), default="sgd",
+                    help="sgd: momentum 0.9; adamw: torch.optim.AdamW's defaults but --lr; lamb: "
+                         "MasterWeightLAMB's defaults but --lr, no weight decay on 1-D parameters "
+                         "(needs --master-weights)")
     ap.add_argument("--clip-grad-norm", type=float, default=None, metavar="X",
                     help="clip the global gradient L2 norm at X: max_grad_norm=X with "
                          "--master-weights, else torch.nn.utils.clip_grad_norm_ between the "
@@ -79,6 +81,8 @@ def main() -> int:
     a = ap.parse_args()
     if a.loss_scale and not a.master_weights:
         ap.error("--loss-scale needs --master-weights: stock GradScaler refuses f16 gradients")
+    if a.optimizer == "lamb" and not a.master_weights:
+        ap.error("--optimizer lamb needs --master-weights: torch.optim has no LAMB")
 
     t_proc = time.time()
     import torch
@@ -99,13 +103,18 @@ def main() -> int:
     name = os.environ.get("TOK8S_REPLICA", "replica-%d" % rep.rank)
     edp = ElasticDataParallel(model, rep.comm, bucket_cap_mb=25)
     if a.master_weights:
-        from torch_on_k8s_b200.optim import DynamicLossScale, MasterWeightAdamW, MasterWeightSGD
+        from torch_on_k8s_b200.optim import (DynamicLossScale, MasterWeightAdamW, MasterWeightLAMB,
+                                             MasterWeightSGD, lamb_param_groups)
         ls = DynamicLossScale() if a.loss_scale else None
-        opt = MasterWeightAdamW(model.parameters(), lr=a.lr, max_grad_norm=a.clip_grad_norm,
-                                loss_scale=ls) \
-            if a.optimizer == "adamw" else \
-            MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9,
-                            max_grad_norm=a.clip_grad_norm, loss_scale=ls)
+        if a.optimizer == "lamb":
+            opt = MasterWeightLAMB(lamb_param_groups(model.parameters()), lr=a.lr,
+                                   max_grad_norm=a.clip_grad_norm, loss_scale=ls)
+        elif a.optimizer == "adamw":
+            opt = MasterWeightAdamW(model.parameters(), lr=a.lr, max_grad_norm=a.clip_grad_norm,
+                                    loss_scale=ls)
+        else:
+            opt = MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9,
+                                  max_grad_norm=a.clip_grad_norm, loss_scale=ls)
     else:
         opt = torch.optim.AdamW(model.parameters(), lr=a.lr) if a.optimizer == "adamw" else \
             torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
