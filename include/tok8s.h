@@ -246,6 +246,20 @@ int tok_bn2_add_relu_bwd(const void* gy, const void* y, const void* x, const flo
                          void* grad_weight_d, void* grad_bias_d, int64_t rows, int channels,
                          void* workspace, void* cuda_stream);
 
+/* Max pool with kernel 3, stride 2, padding 1 (ResNet's stem; torch_on_k8s_b200/fused_bn.py's
+ * max_pool) of an NHWC bf16 activation [n, h, w, channels], bit-identical to ATen's channels_last
+ * max_pool2d and its backward.  The pooled output y is [n, oh, ow, channels] with oh = (h - 1) / 2 + 1,
+ * ow = (w - 1) / 2 + 1; `positions` (uint8, laid out as y) records for every pooled element which of
+ * the 9 window positions (kh * 3 + kw) won, or 255 when ATen's index lies outside the window.
+ * tok_max_pool_bwd writes every element of dx [n, h, w, channels] from gy (laid out as y) and those
+ * positions.  Activations must be 16-byte aligned, positions 8-byte aligned and channels a multiple
+ * of 8 (TOK_ERR_ALIGN); n * h * w * channels must stay below 2^31 (TOK_ERR_INVALID).  Enqueued on
+ * `cuda_stream` (one launch), no synchronisation; TOK_ERR_NO_DEVICE without a GPU. */
+int tok_max_pool_fwd(const void* x, void* y, void* positions, int64_t n, int64_t h, int64_t w,
+                     int channels, void* cuda_stream);
+int tok_max_pool_bwd(const void* gy, const void* positions, void* dx, int64_t n, int64_t h,
+                     int64_t w, int channels, void* cuda_stream);
+
 /* SGD step on fp32 master weights for bf16 / f16 parameters (torch_on_k8s_b200/optim.py), one launch
  * per gradient bucket.  For every element of every segment it produces the bits of
  *   torch.optim.SGD(masters, lr, momentum, dampening, weight_decay, nesterov).step()   (foreach)

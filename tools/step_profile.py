@@ -29,6 +29,8 @@ CATEGORIES = [
     # libtok8s' fused batch-norm apply (+ add + ReLU) counts as BN apply, not as a tok kernel
     ("bn_apply", re.compile(r"batch_norm_transform_input|batch_norm_elemt|bn_fused")),
     ("bn_backward", re.compile(r"bn_bwd_")),
+    # libtok8s' stem max pool counts where ATen's did
+    ("other", re.compile(r"max_pool")),
     ("tok", re.compile(r"\btok::")),
     ("bn_stats", re.compile(r"batch_norm_collect_statistics|batch_norm_update_stats|"
                             r"batch_norm_stats|welford")),

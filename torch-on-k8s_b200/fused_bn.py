@@ -30,6 +30,13 @@ The fused path is taken when the inputs allow it: CUDA, bf16 activations and bat
 channels_last-contiguous 4-D activations with C % 8 == 0 and 16-byte aligned data, a module in
 training mode that tracks running statistics with a fixed momentum.  Anything else (CPU, eval, fp32,
 NCHW, ...) runs the stock composition.
+
+    max_pool(x, pool)              == pool(x)
+
+runs ResNet's stem max pool (an nn.MaxPool2d with kernel 3, stride 2, padding 1) through libtok8s's
+pool kernels on activations the batch-norm kernels accept, bit-identical to ATen's output and
+gradient; it saves one position byte per pooled element where ATen saves the input and an int64
+index.  Any other pool or input calls the module.
 """
 from __future__ import annotations
 
@@ -224,6 +231,56 @@ def _fused_backward(ctx, gy, need, saved):
             return dx, dw, db, dxd, dwd, dbd, None, None, None
     _ffi.check(rc)
     return grads + (None,) * 5
+
+
+def _stem_pool(pool: torch.nn.Module) -> bool:
+    pair = torch.nn.modules.utils._pair
+    return (isinstance(pool, torch.nn.MaxPool2d) and pair(pool.kernel_size) == (3, 3)
+            and pair(pool.stride) == (2, 2) and pair(pool.padding) == (1, 1)
+            and pair(pool.dilation) == (1, 1) and not pool.ceil_mode and not pool.return_indices)
+
+
+class _MaxPool(torch.autograd.Function):
+    """ResNet's stem max pool (3x3, stride 2, padding 1) through libtok8s; saves one position byte per
+    pooled element where ATen saves its input and an int64 index."""
+
+    @staticmethod
+    def forward(ctx, x):
+        n, ch, h, w = x.shape
+        y = torch.empty((n, ch, (h - 1) // 2 + 1, (w - 1) // 2 + 1), dtype=x.dtype, device=x.device,
+                        memory_format=torch.channels_last)
+        pos = torch.empty((n, y.shape[2], y.shape[3], ch), dtype=torch.uint8, device=x.device)
+        with torch.cuda.device(x.device):
+            stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
+            rc = _ffi.lib().tok_max_pool_fwd(_ptr(x), _ptr(y), _ptr(pos), n, h, w, ch, stream)
+        _ffi.check(rc)
+        ctx.save_for_backward(pos)
+        ctx.in_shape = x.shape
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        (pos,) = ctx.saved_tensors
+        n, ch, h, w = ctx.in_shape
+        if not _fusable_act(gy):
+            gy = gy.clone(memory_format=torch.channels_last)  # e.g. the zero-stride gy of y.sum()
+        dx = torch.empty((n, ch, h, w), dtype=gy.dtype, device=gy.device,
+                         memory_format=torch.channels_last)
+        with torch.cuda.device(gy.device):
+            stream = C.c_void_p(torch.cuda.current_stream(gy.device).cuda_stream)
+            rc = _ffi.lib().tok_max_pool_bwd(_ptr(gy), _ptr(pos), _ptr(dx), n, h, w, ch, stream)
+        _ffi.check(rc)
+        return dx
+
+
+def max_pool(x: torch.Tensor, pool: torch.nn.Module) -> torch.Tensor:
+    """pool(x) for an nn.MaxPool2d; through libtok8s for ResNet's stem configuration (kernel 3,
+    stride 2, padding 1, no dilation, ceil_mode or return_indices) on CUDA bf16 channels_last
+    inputs, bit-identical to ATen's output and gradient."""
+    if _stem_pool(pool) and _fusable_act(x):
+        return _MaxPool.apply(x)
+    return pool(x)
 
 
 def bn_relu(x: torch.Tensor, bn: torch.nn.Module) -> torch.Tensor:

@@ -4,13 +4,14 @@ network for checkpoints).
 
 Every batch norm is applied through torch_on_k8s_b200.fused_bn together with the ReLU and residual
 add that follow it: on CUDA bf16 channels_last training inputs that is one fused libtok8s kernel
-per site, bit-identical to the unfused ops; anything else runs the plain nn composition."""
+per site, bit-identical to the unfused ops; anything else runs the plain nn composition.  The stem's
+max pool runs through fused_bn.max_pool under the same conditions."""
 from __future__ import annotations
 
 import torch
 import torch.nn as nn
 
-from torch_on_k8s_b200.fused_bn import bn2_add_relu, bn_add_relu, bn_relu
+from torch_on_k8s_b200.fused_bn import bn2_add_relu, bn_add_relu, bn_relu, max_pool
 
 
 class Bottleneck(nn.Module):
@@ -72,7 +73,7 @@ class ResNet50(nn.Module):
         return nn.Sequential(*layers)
 
     def forward(self, x):
-        x = self.maxpool(bn_relu(self.conv1(x), self.bn1))
+        x = max_pool(bn_relu(self.conv1(x), self.bn1), self.maxpool)
         x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
         x = torch.flatten(self.avgpool(x), 1)
         return self.fc(x)
