@@ -430,6 +430,43 @@ int tok_lamb_master_step(const tok_lamb_segment_t* segments, int count, int64_t 
                          double step, float* partials, const float* inv_scale,
                          const float* grad_coef, void* cuda_stream);
 
+/* LARS step on fp32 master weights for bf16 / f16 parameters (torch_on_k8s_b200/optim.py's
+ * MasterWeightLARS): apex LARC's algorithm around torch.optim.SGD, for the parameters of one param
+ * group that share a momentum state.  For every segment it produces the bits of the torch loop on the
+ * fp32 masters W, with B the momentum buffers and G = f32(grad):
+ *   wn, gn = _foreach_norm(W), _foreach_norm(G)          (W before this step's update)
+ *   r = trust_coefficient * wn / (gn + wn * weight_decay + eps)
+ *   r = clamp(r / lr, max=1)                             (clip != 0; NaN stays NaN)
+ *   G = where(wn != 0 & gn != 0, (G + weight_decay * W) * r, G)
+ *   SGD(W, lr, momentum, dampening, weight_decay=0, nesterov).step();  param.copy_(W)     (RNE)
+ * with ATen's roundings for 0-d fp32 tensors and Python scalars: a multiply by float(scalar) is one
+ * rounding and `r / lr` is r * float(1.0 / lr), so a clipped ratio is 1 at lr = 0.  `fresh` says
+ * the momentum buffers hold nothing yet (B = G on this step), as for tok_sgd_master_step; `momentum`
+ * NULL in the segments when momentum == 0.  With `inv_scale` not NULL, G = f32(grad) * *inv_scale (one
+ * rounding); with `grad_coef` not NULL, G = G * *grad_coef follows (one more rounding):
+ * tok_sgd_master_step_unscaled's gradient.  Both are DEVICE fp32 scalars.  The table follows
+ * tok_grad_norms's rules (TOK_NORM_CHUNK elements per chunk, one CTA per chunk, a DEVICE array): both
+ * norms keep _foreach_norm's chunking and reduction trees.  `partials` is DEVICE fp32 scratch of
+ * 2 * `chunks` elements.  Two launches, none when `chunks` is 0: the first writes each chunk's partial
+ * sums of W^2 and G^2; the second reduces a segment's partials in each of its CTAs and updates W, B
+ * and param.  Returns TOK_ERR_INVALID for a null or empty table, a negative or too large `chunks`, a
+ * dtype other than TOK_BF16 / TOK_F16, a negative or non-finite lr, momentum, dampening, weight_decay,
+ * trust_coefficient or eps, nesterov without a momentum or with dampening, null partials with chunks,
+ * TOK_ERR_NO_DEVICE without a GPU.  Enqueued on `cuda_stream`, no synchronisation. */
+typedef struct tok_lars_segment {
+  const void* grad;   /* bf16 / f16[numel], the parameter's gradient (anywhere in its bucket)     */
+  void* param;        /* bf16 / f16[numel], written                                               */
+  float* master;      /* fp32[numel], dense, read and written                                     */
+  float* momentum;    /* fp32[numel], dense, read and written; NULL when momentum == 0           */
+  int64_t numel;
+  int64_t chunk0;     /* index of this segment's first chunk, counted in TOK_NORM_CHUNKs          */
+} tok_lars_segment_t;
+int tok_lars_master_step(const tok_lars_segment_t* segments, int count, int64_t chunks, int dtype,
+                         double lr, double momentum, double dampening, double weight_decay,
+                         int nesterov, int fresh, double trust_coefficient, int clip, double eps,
+                         float* partials, const float* inv_scale, const float* grad_coef,
+                         void* cuda_stream);
+
 /* Which algorithm AUTO picks for `wire_bytes` on this communicator. */
 int tok_allreduce_algo(tok_comm_t* comm, size_t wire_bytes, int* algo);
 /* Number of kernels this communicator has launched so far (bench.py's gpu_launches): exchange,

@@ -86,15 +86,7 @@ __device__ __forceinline__ void norm_partial(const tok_norm_segment_t* __restric
   __shared__ tok_norm_segment_t s;
   __shared__ float red[32];
   const int64_t c = blockIdx.x;
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = count - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (seg[mid].chunk0 <= c) lo = mid; else hi = mid - 1;
-    }
-    s = seg[lo];
-  }
-  __syncthreads();
+  find_segment(seg, count, c, s);
   const int64_t start = (c - s.chunk0) * kNormChunk;
   const int64_t n = min(s.numel - start, kNormChunk);   // this chunk's elements
   const uint16_t* x = (const uint16_t*)s.grad + start;
@@ -199,15 +191,7 @@ __global__ void __launch_bounds__(kVoteThreads)
                      float* __restrict__ found_inf) {
   __shared__ tok_norm_segment_t s;
   const int64_t c = blockIdx.x;
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = count - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (seg[mid].chunk0 <= c) lo = mid; else hi = mid - 1;
-    }
-    s = seg[lo];
-  }
-  __syncthreads();
+  find_segment(seg, count, c, s);
   const int64_t start = (c - s.chunk0) * kNormChunk;
   const int64_t n = min(s.numel - start, kNormChunk);
   const uint16_t* x = (const uint16_t*)s.grad + start;

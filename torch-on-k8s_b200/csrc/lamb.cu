@@ -77,21 +77,6 @@ __device__ __forceinline__ float lamb_update(const LambArgs& a, float m, float v
   return a.use_wd ? __fmaf_rn(a.wd, w, u) : u;
 }
 
-// Thread 0 finds the last segment whose first chunk is <= the block's and copies it to `s`.
-__device__ __forceinline__ void find_segment(const LambArgs& a, int64_t c, tok_lamb_segment_t& s) {
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = a.count - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (a.seg[mid].chunk0 <= c) lo = mid; else hi = mid - 1;
-    }
-    s = a.seg[lo];
-  }
-  __syncthreads();
-}
-
-__device__ __forceinline__ bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
-
 template <typename T, bool kClip, bool kUnscale>
 __global__ void __launch_bounds__(kNormThreads)
     lamb_moments_kernel(const LambArgs a, const float* __restrict__ inv_scale,
@@ -99,7 +84,7 @@ __global__ void __launch_bounds__(kNormThreads)
   __shared__ tok_lamb_segment_t s;
   __shared__ float red[32];
   const int64_t c = blockIdx.x;
-  find_segment(a, c, s);
+  find_segment(a.seg, a.count, c, s);
   const float inv = kUnscale ? __ldg(inv_scale) : 1.0f;
   const float coef = kClip ? __ldg(grad_coef) : 1.0f;
   const int64_t start = (c - s.chunk0) * kLambChunk;
@@ -203,7 +188,7 @@ __global__ void __launch_bounds__(kNormThreads) lamb_apply_kernel(const LambArgs
   __shared__ float red[32];
   __shared__ float ratio_lr;
   const int64_t c = blockIdx.x;
-  find_segment(a, c, s);
+  find_segment(a.seg, a.count, c, s);
   float lr_c = a.lr;   // `* lr`, or with the trust ratio `where(...) * lr`
   if (a.use_wd) {
     const int64_t nchunks = (s.numel + kLambChunk - 1) / kLambChunk;

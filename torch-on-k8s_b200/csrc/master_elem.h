@@ -1,6 +1,7 @@
-// Per-element pieces of the fp32 master-weight steps, shared by SGD / Adam (optim.cu) and LAMB
-// (lamb.cu): the half-precision conversions, the gradient as the optimizer reads it, and the roundings
-// of torch's Adam moment update.  optim.cu's header comment says how each rounding was settled.
+// Per-element pieces of the fp32 master-weight steps, shared by SGD / Adam (optim.cu), LAMB (lamb.cu)
+// and LARS (lars.cu): the half-precision conversions, the gradient as the optimizer reads it, the
+// roundings of torch's Adam moment update and torch's SGD element step.  optim.cu's header comment
+// says how each rounding was settled.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -48,6 +49,25 @@ __device__ __forceinline__ float second_moment(float v, float g, float beta2, fl
   v = __fmul_rn(v, beta2);
   return value == 1.0f ? __fmaf_rn(g, g, v) : __fmaf_rn(value, __fmul_rn(g, g), v);
 }
+
+__device__ __forceinline__ float add_alpha(float a, float b, float alpha) {
+  return __fmaf_rn(alpha, b, a);   // a + alpha * b, one rounding (optim.cu's header comment)
+}
+
+// torch.optim.SGD's foreach step on one element of the masters: returns the new master w and updates
+// the momentum buffer m in place (m is neither read nor written without use_mu, nor read when fresh).
+__device__ __forceinline__ float sgd_update(float g, float w, float& m, float neg_lr, float mu,
+                                            float damp_alpha, float wd, bool use_wd, bool use_mu,
+                                            bool nesterov, bool fresh) {
+  if (use_wd) g = add_alpha(g, w, wd);
+  if (use_mu) {
+    m = fresh ? g : add_alpha(__fmul_rn(m, mu), g, damp_alpha);
+    g = nesterov ? add_alpha(g, m, mu) : m;
+  }
+  return add_alpha(w, g, neg_lr);
+}
+
+__device__ __forceinline__ bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
 
 }  // namespace
 }  // namespace tok

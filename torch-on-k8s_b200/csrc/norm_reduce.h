@@ -1,5 +1,5 @@
 // ATen's block reductions for the fp32 L2 norms of torch._foreach_norm, shared by the gradient norms
-// (grad_norm.cu) and LAMB's trust ratios (lamb.cu).  See grad_norm.cu's header comment for how they
+// (grad_norm.cu) and the trust ratios of LAMB (lamb.cu) and LARS (lars.cu).  See grad_norm.cu's header comment for how they
 // were read off torch 2.11's LpNormFunctor and lpnorm_cleanup.
 #pragma once
 #include <cuda_runtime.h>
@@ -34,6 +34,21 @@ __device__ __forceinline__ float cleanup_sum(const float* __restrict__ partials,
   float val = 0.0f;
   for (int64_t i = threadIdx.x; i < nchunks; i += kNormThreads) val = __fadd_rn(val, partials[i]);
   return block_sum(val, shared);
+}
+
+// The segment of chunk c in a table of `count` segments with first-chunk indices `chunk0`: thread 0
+// finds the last segment whose first chunk is <= c and copies it to `s`, then the block syncs.
+template <typename Seg>
+__device__ __forceinline__ void find_segment(const Seg* seg, int count, int64_t c, Seg& s) {
+  if (threadIdx.x == 0) {
+    int lo = 0, hi = count - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (seg[mid].chunk0 <= c) lo = mid; else hi = mid - 1;
+    }
+    s = seg[lo];
+  }
+  __syncthreads();
 }
 
 }  // namespace

@@ -72,6 +72,7 @@
 #include <stdint.h>
 
 #include "master_elem.h"
+#include "norm_reduce.h"
 #include "tok_internal.h"
 
 namespace tok {
@@ -80,10 +81,6 @@ namespace {
 constexpr int kSgdThreads = 256;            // threads per CTA of both kernels
 constexpr int64_t kChunk = TOK_SGD_CHUNK;   // elements per (segment, chunk) work item
 static_assert(kChunk % 8 == 0, "a chunk must start at a vector boundary of every array");
-
-__device__ __forceinline__ float add_alpha(float a, float b, float alpha) {
-  return __fmaf_rn(alpha, b, a);   // a + alpha * b, one rounding (see the header comment)
-}
 
 __device__ __forceinline__ float lane(const float4& v, int k) {
   return k == 0 ? v.x : k == 1 ? v.y : k == 2 ? v.z : v.w;
@@ -126,15 +123,7 @@ template <typename T, bool kClip, bool kUnscale, typename Step>
 __device__ __forceinline__ void walk_chunk(const Step& a, float coef, float inv_scale) {
   __shared__ typename Step::Segment s;
   const int64_t c = blockIdx.x;
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = a.count - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (a.seg[mid].chunk0 <= c) lo = mid; else hi = mid - 1;
-    }
-    s = a.seg[lo];
-  }
-  __syncthreads();
+  find_segment(a.seg, a.count, c, s);
   const int64_t start = (c - s.chunk0) * kChunk;
   const int64_t end = min(start + kChunk, s.numel);
   if (start >= end) return;
@@ -168,12 +157,7 @@ struct SgdArgs {
 
   // One element: returns the new master; updates m in place.
   __device__ __forceinline__ float step(float g, float w, float& m) const {
-    if (use_wd) g = add_alpha(g, w, wd);
-    if (use_mu) {
-      m = fresh ? g : add_alpha(__fmul_rn(m, mu), g, damp_alpha);
-      g = nesterov ? add_alpha(g, m, mu) : m;
-    }
-    return add_alpha(w, g, neg_lr);
+    return sgd_update(g, w, m, neg_lr, mu, damp_alpha, wd, use_wd, use_mu, nesterov, fresh);
   }
 
   __device__ __forceinline__ bool vectorizable(const tok_sgd_segment_t& s, int64_t i) const {

@@ -24,8 +24,8 @@ class BucketAllreduceHook:
     overlaps the backward kernels that are still producing bucket k+1 (DDP's own overlap model);
     the returned CUDA-aware Future carries the event consumers must wait on.
 
-    optimizer (a MasterWeightSGD, MasterWeightAdam, MasterWeightAdamW or MasterWeightLAMB): each
-    bucket's optimizer step is enqueued on the same stream right behind its exchange, before the
+    optimizer (a MasterWeightSGD, MasterWeightAdam, MasterWeightAdamW, MasterWeightLAMB or
+    MasterWeightLARS): each bucket's optimizer step is enqueued on the same stream right behind its exchange, before the
     Future is set; optimizer.step() then only orders the current stream after that stream.  An
     optimizer with max_grad_norm enqueues only the bucket's gradient norms there; its step() forms
     the global norm and steps every bucket.  One with a loss scale enqueues only the bucket's inf /

@@ -90,9 +90,9 @@ class ElasticDataParallel(torch.nn.Module):
 
     def reduce_grads(self, stream: Optional[torch.cuda.Stream] = None, optimizer=None) -> None:
         """Average the gradient buckets across the current peer group (in place, zero-copy).
-        optimizer (a MasterWeightSGD, MasterWeightAdam, MasterWeightAdamW or MasterWeightLAMB): each
-        bucket's step is enqueued right behind its exchange; optimizer.step() then launches nothing
-        for these parameters.  With max_grad_norm only the bucket's gradient norms are enqueued there, and
+        optimizer (a MasterWeightSGD, MasterWeightAdam, MasterWeightAdamW, MasterWeightLAMB or
+        MasterWeightLARS): each bucket's step is enqueued right behind its exchange; optimizer.step()
+        then launches nothing for these parameters.  With max_grad_norm only the bucket's gradient norms are enqueued there, and
         optimizer.step() steps every bucket once the global norm exists.  With a loss scale only the
         bucket's inf / NaN check (or its unscaled norms) is enqueued there, and optimizer.step()
         steps every bucket unless an inf or NaN was found."""

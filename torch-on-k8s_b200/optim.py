@@ -1,5 +1,5 @@
-"""SGD, Adam, AdamW and LAMB on fp32 master weights for bf16 / f16 models, stepped by libtok8s kernels
-per bucket.
+"""SGD, Adam, AdamW, LAMB and LARS on fp32 master weights for bf16 / f16 models, stepped by libtok8s
+kernels per bucket.
 
 bf16 keeps 8 significant bits: `torch.optim.SGD` on bf16 parameters rounds away every update smaller
 than about 1/256 of the weight, and an Adam update is at most about `lr`.  These optimizers keep, per
@@ -14,7 +14,7 @@ under torch's keys, and one step produces the bits of
 in a single pass over gradient, master, optimizer state and parameter (csrc/optim.cu).
 MasterWeightSGD keeps `momentum_buffer`; MasterWeightAdam and MasterWeightAdamW keep `exp_avg`,
 `exp_avg_sq`, `max_exp_avg_sq` (amsgrad) and a CPU float32 `step`, as torch does; MasterWeightLAMB
-keeps the same keys but `max_exp_avg_sq`.
+keeps the same keys but `max_exp_avg_sq`; MasterWeightLARS keeps SGD's `momentum_buffer`.
 
 MasterWeightLAMB is LAMB (You et al., 2019) as apex FusedLAMB runs it in its defaults (adam_w_mode,
 bias_correction, grad_averaging, use_nvlamb=False).  torch has no LAMB, so this is the restatement it
@@ -42,6 +42,38 @@ parameter's own step count, in Python doubles, as torch's Adam computes them.  T
 Unlike apex, clipping is clip_grad_norm_'s max_grad_norm= below, and the defaults are lr=1e-3,
 betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01.  The trust ratio is per parameter, so a bucket's full
 LAMB step runs behind its own exchange, as Adam's does.
+
+MasterWeightLARS is LARS (You et al., 2017) as apex LARC runs it around torch.optim.SGD, in its
+clip=True and clip=False modes.  torch has no LARS, so this is the restatement it matches bit for bit,
+per param group, on the masters W with momentum buffers B and G the fp32 master.grad (as for LAMB):
+
+    # groups with lars=True
+    wn, gn = torch._foreach_norm(W), torch._foreach_norm(G)   # W before this step's update
+    for w, g, a, b in zip(W, G, wn, gn):
+        r = trust_coefficient * a / (b + a * weight_decay + eps)
+        if clip:
+            r = torch.clamp(r / lr, max=1.0)      # LARC's min(r / lr, 1), NaN included
+        g.copy_(torch.where((a != 0) & (b != 0), (g + weight_decay * w) * r, g))
+    torch.optim.SGD(W, lr, momentum, dampening, weight_decay=0.0, nesterov=nesterov,
+                    foreach=True).step()          # momentum_buffer state, first step clones g
+    P.copy_(W)                                    # round to nearest even into bf16 / f16
+    # groups with lars=False: MasterWeightSGD's step, with the group's own weight_decay
+
+Where it differs from apex LARC, and why:
+  * The norms are _foreach_norm's, which the kernels reproduce bit for bit (csrc/grad_norm.cu).
+    LARC's per-tensor torch.norm uses ATen's generic reduction, whose order can change the last bits.
+  * LARC's host `if param_norm != 0 and grad_norm != 0` is a torch.where: no host sync per tensor.
+  * The per-group key `lars` (default True) lets batch-norm and bias parameters skip the adaptation
+    and the decay, as MLPerf's ResNet-50 does (lars_param_groups); LARC has no such key.
+  * The defaults are LARC's: trust_coefficient=0.02, clip=True, eps=1e-8.
+Weight decay is LARC's, not SGD's: g + (wd * w), two roundings rather than _foreach_add_'s one FMA,
+applied only where both norms are non-zero (a tensor with a zero norm gets neither the ratio nor any
+decay), and the SGD step runs with weight_decay = 0.  The ratio's roundings are ATen's for 0-d fp32
+CUDA tensors and Python scalars: `trust_coefficient * a` and `a * weight_decay` are one multiply by
+the float, and `r / lr` is a multiply by the reciprocal float(1.0 / lr) (div_true_kernel_cuda's
+CPU-scalar path, settled on an H100 by tools/scalar_div_probe.py), so at lr = 0 a clipped ratio is 1.
+Two kernels per launch (csrc/lars.cu): the chunk partials of both norms, then the ratio, the
+transform and SGD's element step.
 
 Used on its own, step() steps every parameter that has a gradient.  Handed to
 `Replica.wrap(..., optimizer=opt)` or `ElasticDataParallel.reduce_grads(optimizer=opt)`, the step of
@@ -119,9 +151,10 @@ def _dense(t: torch.Tensor) -> bool:
 
 
 def segment_table(entries, chunk: int = CHUNK) -> Tuple[List[tuple], int]:
-    """Rows of tok_sgd_segment_t / tok_adam_segment_t / tok_lamb_segment_t — (grad, param, *fp32
-    state, numel, chunk0) as integers, 0 for a None state tensor — for [(grad, param, *fp32 state)],
-    and the total number of chunks of `chunk` elements (NORM_CHUNK for LAMB)."""
+    """Rows of tok_sgd_segment_t / tok_adam_segment_t / tok_lamb_segment_t / tok_lars_segment_t —
+    (grad, param, *fp32 state, numel, chunk0) as integers, 0 for a None state tensor — for
+    [(grad, param, *fp32 state)], and the total number of chunks of `chunk` elements (NORM_CHUNK for
+    LAMB and LARS)."""
     rows, chunks = [], 0
     for g, p, *state in entries:
         n = p.numel()
@@ -308,6 +341,10 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         `inv_scale` (the device inverse loss scale) the unscaled one, clipped too with `coef`."""
         raise NotImplementedError
 
+    def _chunk(self, group: dict) -> int:
+        """Elements per chunk of the tables _kernel takes for `group`."""
+        return self._CHUNK
+
     def _table(self, key: tuple, rows: List[tuple], dev: torch.device) -> torch.Tensor:
         cached = self._tables.get(key)
         if cached is None or cached[0] != rows:
@@ -342,7 +379,7 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             if not entries:
                 continue
             dev = entries[0][1].device
-            rows, chunks = segment_table(entries, self._CHUNK)
+            rows, chunks = segment_table(entries, self._chunk(group))
             table = self._table(key + (sub,), rows, dev)
             with torch.cuda.device(dev):
                 self._kernel(group, table, len(rows), chunks, _DTYPES[entries[0][1].dtype], arg,
@@ -767,3 +804,89 @@ def lamb_param_groups(params: Iterable[torch.Tensor], weight_decay: float = 1e-2
     params = list(params)
     return [dict(params=[p for p in params if p.dim() > 1], weight_decay=weight_decay),
             dict(params=[p for p in params if p.dim() <= 1], weight_decay=0.0)]
+
+
+def _check_lars_group(group: dict) -> None:
+    """torch.optim.SGD's checks and messages, then the LARS keys and what the kernel cannot take."""
+    for k in ("lr", "momentum", "dampening", "weight_decay", "trust_coefficient", "eps"):
+        if isinstance(group[k], (bool, torch.Tensor)) or not isinstance(group[k], (int, float)):
+            raise ValueError("MasterWeightLARS takes %s as a Python float, got %r" % (k, group[k]))
+    if group["lr"] < 0.0:
+        raise ValueError(f"Invalid learning rate: {group['lr']}")
+    if group["momentum"] < 0.0:
+        raise ValueError(f"Invalid momentum value: {group['momentum']}")
+    if group["weight_decay"] < 0.0:
+        raise ValueError(f"Invalid weight_decay value: {group['weight_decay']}")
+    if group["nesterov"] and (group["momentum"] <= 0 or group["dampening"] != 0):
+        raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+    for k in ("lr", "momentum", "dampening", "weight_decay", "trust_coefficient", "eps"):
+        if not (math.isfinite(group[k]) and group[k] >= 0.0):
+            raise ValueError(f"Invalid {k} value: {group[k]}")
+    for k in ("clip", "lars"):
+        if not isinstance(group[k], bool):
+            raise ValueError(f"Invalid {k} value: {group[k]!r} (a bool)")
+
+
+class MasterWeightLARS(_MasterWeightOptimizer):
+    """LARS (You et al., 2017) on fp32 masters: apex LARC's algorithm around torch.optim.SGD, restated
+    with torch ops in the module docstring.  It keeps MasterWeightSGD's state keys, so its state_dict
+    loads into a stock SGD.  `trust_coefficient`, `clip`, `eps` and `lars` are per-group keys; a group
+    with `lars=False` takes MasterWeightSGD's step with its own weight_decay.  Each bucket (or param
+    group) takes its full step behind its own exchange: the trust ratio needs the norms of one
+    parameter's master and gradient, not a global norm."""
+
+    _FP32_STATE = ("master_param", "momentum_buffer")
+    _FP32_HINT = "torch.optim has no LARS to use instead"
+
+    def __init__(self, params, lr: float, momentum: float = 0.0, dampening: float = 0.0,
+                 weight_decay: float = 0.0, nesterov: bool = False, *,
+                 trust_coefficient: float = 0.02, clip: bool = True, eps: float = 1e-8,
+                 max_grad_norm: Optional[float] = None, error_if_nonfinite: bool = False,
+                 loss_scale: Optional[DynamicLossScale] = None):
+        defaults = dict(lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay,
+                        nesterov=nesterov, trust_coefficient=trust_coefficient, clip=clip, eps=eps,
+                        lars=True)
+        _check_lars_group(defaults)
+        super().__init__(params, defaults, max_grad_norm, error_if_nonfinite, loss_scale)
+
+    def add_param_group(self, param_group: dict) -> None:
+        super().add_param_group(param_group)
+        try:
+            _check_lars_group(self.param_groups[-1])
+        except ValueError:
+            group = self.param_groups.pop()
+            for p in group["params"]:
+                self._group_of.pop(id(p), None)
+                self._slot_of.pop(id(p), None)
+                self.state.pop(p, None)
+            raise
+
+    def _chunk(self, group: dict) -> int:
+        # _foreach_norm's chunks where the trust ratio's norms keep its reduction
+        return NORM_CHUNK if group["lars"] else CHUNK
+
+    _split = MasterWeightSGD._split   # one launch per momentum state: fresh buffers, then the rest
+
+    def _kernel(self, group, table, count, chunks, dtype, fresh, stream, coef, inv_scale) -> None:
+        if not group["lars"]:
+            MasterWeightSGD._kernel(self, group, table, count, chunks, dtype, fresh, stream, coef,
+                                    inv_scale)
+            return
+        # caching-allocator scratch on `stream` (current): the two norm partials of every chunk
+        partials = torch.empty(2 * chunks, dtype=torch.float32, device=table.device)
+        _ffi.check(_ffi.lib().tok_lars_master_step(
+            C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], group["momentum"],
+            group["dampening"], group["weight_decay"], int(group["nesterov"]), fresh,
+            group["trust_coefficient"], int(group["clip"]), group["eps"],
+            C.c_void_p(partials.data_ptr()),
+            C.c_void_p(0 if inv_scale is None else inv_scale.data_ptr()),
+            C.c_void_p(0 if coef is None else coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
+
+
+def lars_param_groups(params: Iterable[torch.Tensor], weight_decay: float = 5e-5) -> List[dict]:
+    """Large-batch ResNet-50's two LARS param groups, as MLPerf forms them: the convolution and linear
+    weights with trust ratios and `weight_decay`; the 1-D parameters (batch-norm weights and biases,
+    the classifier's bias) with neither (`lars=False`, plain SGD)."""
+    params = list(params)
+    return [dict(params=[p for p in params if p.dim() > 1], weight_decay=weight_decay),
+            dict(params=[p for p in params if p.dim() <= 1], weight_decay=0.0, lars=False)]

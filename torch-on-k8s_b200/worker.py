@@ -43,8 +43,8 @@ class Replica:
         path, with identical results.  A pool that cannot be created raises rather than change
         kernels silently: pass zero_copy=False to ask for the staged path.
 
-        optimizer (a torch_on_k8s_b200.optim.MasterWeightSGD, MasterWeightAdam, MasterWeightAdamW or
-        MasterWeightLAMB over the model's parameters): the hook steps each bucket's parameters right behind the
+        optimizer (a torch_on_k8s_b200.optim.MasterWeightSGD, MasterWeightAdam, MasterWeightAdamW,
+        MasterWeightLAMB or MasterWeightLARS over the model's parameters): the hook steps each bucket's parameters right behind the
         bucket's exchange; optimizer.step() then launches nothing for them.  With max_grad_norm the
         hook enqueues only the bucket's gradient norms, and optimizer.step() steps every bucket.
         With a loss scale the hook enqueues only the bucket's inf / NaN check (or its unscaled

@@ -39,11 +39,13 @@ def main() -> int:
     ap.add_argument("--master-weights", action="store_true",
                     help="bf16 / f16 models: SGD on fp32 master weights, stepped behind each "
                          "bucket's exchange (torch_on_k8s_b200.optim.MasterWeightSGD, or "
-                         "MasterWeightAdamW / MasterWeightLAMB with --optimizer adamw / lamb)")
-    ap.add_argument("--optimizer", choices=("sgd", "adamw", "lamb"), default="sgd",
+                         "MasterWeightAdamW / MasterWeightLAMB / MasterWeightLARS with "
+                         "--optimizer adamw / lamb / lars)")
+    ap.add_argument("--optimizer", choices=("sgd", "adamw", "lamb", "lars"), default="sgd",
                     help="sgd: lr 0.01, momentum 0.9; adamw: torch.optim.AdamW's defaults; lamb: "
-                         "MasterWeightLAMB's defaults, no weight decay on 1-D parameters (needs "
-                         "--master-weights)")
+                         "MasterWeightLAMB's defaults, no weight decay on 1-D parameters; lars: "
+                         "lr 0.01, momentum 0.9, weight decay 5e-5 and no trust ratio on 1-D "
+                         "parameters (lamb and lars need --master-weights)")
     ap.add_argument("--clip-grad-norm", type=float, default=None, metavar="X",
                     help="clip the global gradient L2 norm at X: max_grad_norm=X with "
                          "--master-weights, else torch.nn.utils.clip_grad_norm_ before opt.step()")
@@ -55,8 +57,9 @@ def main() -> int:
     a = ap.parse_args()
     if a.loss_scale and not a.master_weights:
         ap.error("--loss-scale needs --master-weights: stock GradScaler refuses f16 gradients")
-    if a.optimizer == "lamb" and not a.master_weights:
-        ap.error("--optimizer lamb needs --master-weights: torch.optim has no LAMB")
+    if a.optimizer in ("lamb", "lars") and not a.master_weights:
+        ap.error("--optimizer %s needs --master-weights: torch.optim has no %s"
+                 % (a.optimizer, a.optimizer.upper()))
 
     import torch
     from torch_on_k8s_b200.sampler import ReplicaSampler
@@ -70,11 +73,15 @@ def main() -> int:
         model = model.to(memory_format=torch.channels_last)
     if a.master_weights:
         from torch_on_k8s_b200.optim import (DynamicLossScale, MasterWeightAdamW, MasterWeightLAMB,
-                                             MasterWeightSGD, lamb_param_groups)
+                                             MasterWeightLARS, MasterWeightSGD,
+                                             lamb_param_groups, lars_param_groups)
         ls = DynamicLossScale() if a.loss_scale else None
         if a.optimizer == "lamb":
             opt = MasterWeightLAMB(lamb_param_groups(model.parameters()),
                                    max_grad_norm=a.clip_grad_norm, loss_scale=ls)
+        elif a.optimizer == "lars":
+            opt = MasterWeightLARS(lars_param_groups(model.parameters(), 5e-5), lr=0.01,
+                                   momentum=0.9, max_grad_norm=a.clip_grad_norm, loss_scale=ls)
         elif a.optimizer == "adamw":
             opt = MasterWeightAdamW(model.parameters(), max_grad_norm=a.clip_grad_norm,
                                     loss_scale=ls)
