@@ -80,7 +80,9 @@ def test_resnet50_sites(geom):
 
 RAGGED_C = [8, 16, 24, 40, 64, 2048]
 RAGGED_M = [1, 2, 15, 16, 17, 255, 256, 257, 4095, 4096, 4097, 1791, 1792, 1793, 3584, 3585, 32767,
-            32768, 32769, 802816, 3211264]
+            32768, 32769, 802816, 3211264,
+            # past 2^24, where counts stop being exact in float, up to numel = INT32_MAX - 63 at C = 64
+            (1 << 24) - 1, (1 << 24) + 1, (1 << 24) + 3, 3 * (1 << 23) + 1, (1 << 25) - 1]
 
 
 @pytest.mark.parametrize("ch", RAGGED_C)
@@ -143,6 +145,9 @@ def test_workspace_bytes(tok_lib, geom):
     assert fn(100, 64) == 0
     for _, ch, rows, *_ in RESNET50:
         assert fn(rows, ch) == geom(rows, ch)[3] > 0
+    # the 32-bit limit: numel INT32_MAX - 63 is accepted, INT32_MAX + 1 is not
+    assert fn((1 << 25) - 1, 64) == geom((1 << 25) - 1, 64)[3] > 0
+    assert fn(1 << 25, 64) == _ffi.TOK_ERR_INVALID and "32-bit" in _ffi.last_error()
 
 
 def test_abi_needs_a_gpu(tok_lib):

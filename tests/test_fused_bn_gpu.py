@@ -154,35 +154,94 @@ def test_saved_invstd_matches_native_batch_norm():
     assert_bits(invstd, sinv, "save_invstd")
 
 
-def test_inputs_outside_the_envelope_take_the_stock_path():
+class Spy:
+    """Stands in for the loaded library and records the batch-norm calls."""
+
+    def __init__(self, lib):
+        self.lib, self.calls = lib, []
+
+    def __getattr__(self, name):
+        fn = getattr(self.lib, name)
+        if not name.startswith("tok_bn"):
+            return fn
+        return lambda *a: self.calls.append(name) or fn(*a)
+
+
+@pytest.fixture
+def spy(monkeypatch):
+    from torch_on_k8s_b200 import _ffi
+    s = Spy(_ffi.lib())
+    monkeypatch.setattr(_ffi, "lib", lambda: s)
+    return s
+
+
+def adjust_bn(bn, why):
+    """The module-side conditions the fused path refuses."""
+    if why == "momentum=None":
+        bn.momentum = None  # a cumulative moving average
+    elif why == "affine=False":
+        bn.affine = False
+        bn.weight = bn.bias = None
+    elif why == "track_running_stats=False":
+        bn.track_running_stats = False
+        bn.running_mean = bn.running_var = bn.num_batches_tracked = None
+    elif why == "fp32 parameters":
+        bn.float()  # AMP's layout: fp32 batch norm on bf16 activations
+    return bn
+
+
+def test_inputs_outside_the_envelope_take_the_stock_path(spy):
     need_gpu()
     dev = torch.device("cuda")
     gen = torch.Generator(device=dev).manual_seed(11)
     cases = []
     for kind in (0, 1, 2):
         x = act((4, 16, 6, 6), gen, dev)
+        storage = torch.empty(x.numel() + 1, dtype=BF, device=dev)
+        shifted = storage[1:].view(4, 6, 6, 16).permute(0, 3, 1, 2)  # 2 bytes past 16-byte alignment
+        shifted.copy_(x)
+        assert shifted.is_contiguous(memory_format=CL) and shifted.data_ptr() % 16 == 2
         cases += [
             (kind, x.float(), "fp32"),
             (kind, x.contiguous(), "NCHW"),
             (kind, act((4, 12, 6, 6), gen, dev), "C % 8"),
             (kind, x.cpu(), "CPU"),
             (kind, x, "eval"),
+            (kind, x, "momentum=None"),
+            (kind, x, "affine=False"),
+            (kind, x, "track_running_stats=False"),
+            (kind, x, "fp32 parameters"),
+            (kind, shifted, "misaligned view"),
+            (kind, act((1, 16, 1, 1), gen, dev), "one row"),
         ]
+        if kind:
+            cases.append((kind, x, "residual of another shape"))
     for kind, x, why in cases:
         C = x.shape[1]
         g = torch.Generator(device=dev).manual_seed(1)
-        bn = make_bn(C, g, dev).to(x.device).to(x.dtype)
-        bnd = make_bn(C, g, dev).to(x.device).to(x.dtype) if kind == 2 else None
+        bn = adjust_bn(make_bn(C, g, dev).to(x.device).to(x.dtype), why)
+        bnd = adjust_bn(make_bn(C, g, dev).to(x.device).to(x.dtype), why) if kind == 2 else None
         other = (x * 0.5).contiguous(memory_format=torch.channels_last if x.dim() == 4 and
                                      x.stride(1) == 1 else torch.contiguous_format) if kind else None
+        if why == "residual of another shape":
+            other = act((4, 16, 1, 1), gen, dev)  # broadcast over H and W by the stock add
         if why == "eval":
             bn.eval()
             if bnd is not None:
                 bnd.eval()
+        if why == "one row":  # stock refuses a single value per channel in training
+            errors = []
+            for path in (fused, stock):
+                with pytest.raises(ValueError) as e:
+                    path(kind, x, copy.deepcopy(bn), other, copy.deepcopy(bnd))
+                errors.append(str(e.value))
+            assert errors[0] == errors[1], errors
+            continue
         y1 = fused(kind, x, copy.deepcopy(bn), other, copy.deepcopy(bnd))
         y0 = stock(kind, x, copy.deepcopy(bn), other, copy.deepcopy(bnd))
         assert y1.grad_fn is None or type(y1.grad_fn).__name__ != "_BnAddReluBackward", why
         assert_bits(y1, y0, "stock-path output (%s, kind %d)" % (why, kind))
+    assert spy.calls == []
 
 
 def test_three_resnet50_training_steps_match_the_stock_ops(monkeypatch):

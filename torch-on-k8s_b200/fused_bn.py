@@ -28,8 +28,9 @@ the stock backward: `threshold_backward` on the output (recomputed for bn_relu),
 
 The fused path is taken when the inputs allow it: CUDA, bf16 activations and batch-norm tensors,
 channels_last-contiguous 4-D activations with C % 8 == 0 and 16-byte aligned data, a module in
-training mode that tracks running statistics with a fixed momentum.  Anything else (CPU, eval, fp32,
-NCHW, ...) runs the stock composition.
+training mode that tracks running statistics with a fixed momentum and a positive eps.  Anything
+else (CPU, eval, fp32, NCHW, ...) runs the stock composition, which also raises stock's errors (one
+row per channel, eps <= 0).
 
     max_pool(x, pool)              == pool(x)
 
@@ -52,8 +53,10 @@ _INT32_MAX = (1 << 31) - 1
 
 
 def _fusable_bn(bn: torch.nn.Module, x: torch.Tensor) -> bool:
+    # F.batch_norm refuses eps <= 0 with a ValueError; the stock path raises it
     if not (bn.training and bn.track_running_stats and bn.affine and bn.momentum is not None
-            and bn.running_mean is not None and bn.num_batches_tracked is not None):
+            and bn.running_mean is not None and bn.num_batches_tracked is not None
+            and bn.eps > 0):
         return False
     for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var):
         if t.dtype != torch.bfloat16 or t.device != x.device or not t.is_contiguous():
