@@ -7,46 +7,21 @@ import pytest
 import torch
 import torch.nn as nn
 
+from master_weight import abi_args, needs_a_gpu, refused
+
 NAN, INF = float("nan"), float("inf")
 FAKE = ctypes.c_void_p(512)   # a fake (never dereferenced) device pointer
-
-
-def _sgd(**over):
-    a = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=2, lr=0.1, momentum=0.9,
-             dampening=0.0, weight_decay=1e-4, nesterov=0, fresh=0, inv_scale=FAKE,
-             grad_coef=None, stream=None)
-    a.update(over)
-    return list(a.values())
-
-
-def _adam(**over):
-    a = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=2, lr=1e-3, beta1=0.9,
-             beta2=0.999, eps=1e-8, weight_decay=1e-2, decoupled=1, amsgrad=0, step=1.0,
-             inv_scale=FAKE, grad_coef=FAKE, stream=None)
-    a.update(over)
-    return list(a.values())
-
-
-def _norms(**over):
-    a = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=2, inv_scale=FAKE,
+SGD = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=2, lr=0.1, momentum=0.9,
+           dampening=0.0, weight_decay=1e-4, nesterov=0, fresh=0, inv_scale=FAKE,
+           grad_coef=None, stream=None)
+ADAM = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=2, lr=1e-3, beta1=0.9,
+            beta2=0.999, eps=1e-8, weight_decay=1e-2, decoupled=1, amsgrad=0, step=1.0,
+            inv_scale=FAKE, grad_coef=FAKE, stream=None)
+NORMS = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=2, inv_scale=FAKE,
              partials=ctypes.c_void_p(1024), norms=ctypes.c_void_p(2048),
              found_inf=ctypes.c_void_p(4096), stream=None)
-    a.update(over)
-    return list(a.values())
-
-
-def _check(**over):
-    a = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=2,
+CHECK = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=2,
              found_inf=ctypes.c_void_p(4096), stream=None)
-    a.update(over)
-    return list(a.values())
-
-
-def _refused(tok_lib, name, args, says):
-    from torch_on_k8s_b200 import _ffi
-    assert getattr(tok_lib, name)(*args) == _ffi.TOK_ERR_INVALID
-    msg = _ffi.last_error()
-    assert name + ":" in msg and says in msg, msg
 
 
 @pytest.mark.parametrize("bad, says", [
@@ -58,7 +33,7 @@ def _refused(tok_lib, name, args, says):
     (dict(nesterov=1, momentum=0.0), "nesterov"), (dict(inv_scale=None), "null inv_scale"),
     (dict(inv_scale=None, grad_coef=FAKE), "null inv_scale")])
 def test_sgd_unscaled_abi_rejects_bad_arguments(tok_lib, bad, says):
-    _refused(tok_lib, "tok_sgd_master_step_unscaled", _sgd(**bad), says)
+    refused(tok_lib, "tok_sgd_master_step_unscaled", abi_args(SGD, **bad), says)
 
 
 @pytest.mark.parametrize("bad, says", [
@@ -69,7 +44,7 @@ def test_sgd_unscaled_abi_rejects_bad_arguments(tok_lib, bad, says):
     (dict(inv_scale=None), "null inv_scale"), (dict(inv_scale=None, grad_coef=None),
                                                "null inv_scale")])
 def test_adam_unscaled_abi_rejects_bad_arguments(tok_lib, bad, says):
-    _refused(tok_lib, "tok_adam_master_step_unscaled", _adam(**bad), says)
+    refused(tok_lib, "tok_adam_master_step_unscaled", abi_args(ADAM, **bad), says)
 
 
 @pytest.mark.parametrize("bad, says", [
@@ -79,7 +54,7 @@ def test_adam_unscaled_abi_rejects_bad_arguments(tok_lib, bad, says):
     (dict(inv_scale=None), "null inv_scale"), (dict(norms=None), "null norms"),
     (dict(found_inf=None), "null found_inf"), (dict(partials=None), "null partials")])
 def test_unscaled_norm_abi_rejects_bad_arguments(tok_lib, bad, says):
-    _refused(tok_lib, "tok_grad_norms_unscaled", _norms(**bad), says)
+    refused(tok_lib, "tok_grad_norms_unscaled", abi_args(NORMS, **bad), says)
 
 
 @pytest.mark.parametrize("bad, says", [
@@ -88,24 +63,20 @@ def test_unscaled_norm_abi_rejects_bad_arguments(tok_lib, bad, says):
     (dict(chunks=1 << 31), "segments in"), (dict(dtype=0), "bf16 or f16"),
     (dict(dtype=3), "bf16 or f16"), (dict(found_inf=None), "null found_inf")])
 def test_nonfinite_abi_rejects_bad_arguments(tok_lib, bad, says):
-    _refused(tok_lib, "tok_grad_nonfinite", _check(**bad), says)
+    refused(tok_lib, "tok_grad_nonfinite", abi_args(CHECK, **bad), says)
 
 
 def test_abi_needs_a_gpu(tok_lib):
-    if torch.cuda.is_available():
-        pytest.skip("box has a GPU")
-    from torch_on_k8s_b200 import _ffi
-    calls = [(tok_lib.tok_sgd_master_step_unscaled, _sgd()),
-             (tok_lib.tok_sgd_master_step_unscaled, _sgd(dtype=1, momentum=0.0, grad_coef=FAKE)),
-             (tok_lib.tok_adam_master_step_unscaled, _adam()),
-             (tok_lib.tok_adam_master_step_unscaled, _adam(dtype=1, amsgrad=1, grad_coef=None)),
-             (tok_lib.tok_grad_norms_unscaled, _norms()),
-             (tok_lib.tok_grad_norms_unscaled, _norms(dtype=1, chunks=0, partials=None)),
-             (tok_lib.tok_grad_nonfinite, _check()),
-             (tok_lib.tok_grad_nonfinite, _check(dtype=1, chunks=0))]
-    for fn, args in calls:
-        assert fn(*args) == _ffi.TOK_ERR_NO_DEVICE
-        assert "no CPU fallback" in _ffi.last_error()
+    needs_a_gpu([(tok_lib.tok_sgd_master_step_unscaled, abi_args(SGD)),
+                 (tok_lib.tok_sgd_master_step_unscaled,
+                  abi_args(SGD, dtype=1, momentum=0.0, grad_coef=FAKE)),
+                 (tok_lib.tok_adam_master_step_unscaled, abi_args(ADAM)),
+                 (tok_lib.tok_adam_master_step_unscaled,
+                  abi_args(ADAM, dtype=1, amsgrad=1, grad_coef=None)),
+                 (tok_lib.tok_grad_norms_unscaled, abi_args(NORMS)),
+                 (tok_lib.tok_grad_norms_unscaled, abi_args(NORMS, dtype=1, chunks=0, partials=None)),
+                 (tok_lib.tok_grad_nonfinite, abi_args(CHECK)),
+                 (tok_lib.tok_grad_nonfinite, abi_args(CHECK, dtype=1, chunks=0))])
 
 
 # ---- DynamicLossScale -------------------------------------------------------------------------------

@@ -3,8 +3,7 @@ and optimizer state, the half-precision write-back at its overflow thresholds an
 hyperparameters at their boundaries.
 
 Every step kernel (SGD, Adam / AdamW, LAMB; plain, clipped and unscaled) must give the bits of the
-stock restatements the other suites use (test_master_sgd_gpu, test_master_adam_gpu,
-test_master_lamb_gpu, test_grad_clip_gpu, test_loss_scale_gpu) in parameters, masters,
+stock restatements the other suites use (master_weight.Reference) in parameters, masters,
 momentum_buffer, exp_avg, exp_avg_sq, max_exp_avg_sq, step and grad_norm, raw bits compared, so NaN
 sign and payload and the sign of zero count.
 
@@ -21,12 +20,9 @@ path choice is restated from the real data pointers and every catalogue entry mu
 import numpy as np
 import pytest
 
-from test_grad_clip_gpu import ClipReference, state_mismatches
-from test_loss_scale_gpu import INIT_SCALE, INTERVAL, ScaledReference, new_loss_scale, \
-    scaling_matches
-from test_master_adam_gpu import Reference as AdamReference
-from test_master_lamb_gpu import WD, Reference as LambReference
-from test_master_sgd_gpu import Reference as SgdReference, bits, same_bits, sched
+import harness
+from master_weight import INIT_SCALE, INTERVAL, WD, RefLAMB, Reference, bits, new_loss_scale, \
+    same_bits, sched, scaling_matches, state_mismatches, stock
 
 pytestmark = pytest.mark.gpu
 
@@ -122,11 +118,6 @@ SGD_PATHS = ("head", "vector_grad_aligned", "vector_grad_unaligned", "tail", "al
 # strided scalar one; a parameter 8-byte aligned at a chunk start takes the 4-wide apply.
 LAMB_SEGMENTS = ((4000, 0, 0), (4000, 1, 3), (3001, 0, 0), (3001, 2, 1))
 LAMB_PATHS = ("mapping_vector", "mapping_scalar", "apply_vector", "apply_scalar")
-
-
-def _dtype(name):
-    import torch
-    return {"bf16": torch.bfloat16, "f16": torch.float16}[name]
 
 
 def _signed(values, width):
@@ -346,7 +337,7 @@ def flatten(lays):
 
 
 def sgd_layouts(dev, dtype, n=1, grads=True, masters=MASTER_CATALOGUE, states=STATE_CATALOGUE):
-    return [Layout(dev, _dtype(dtype), SEGMENTS, 10 + k,
+    return [Layout(dev, harness.torch_dtype(dtype), SEGMENTS, 10 + k,
                    grads=GRAD_CATALOGUE[dtype] if grads is True else grads, masters=masters,
                    states=states) for k in range(n)]
 
@@ -390,7 +381,7 @@ def test_sgd_at_edge_values(tok_lib, hp_id, dtype):
     lays = sgd_layouts(torch.device("cuda", 0), dtype, 2 if hp_id == "lr_zero_group" else 1)
     spec = [(lays[0].params, 0.1)] + [(lay.params, 0.0) for lay in lays[1:]]
     opt = MasterWeightSGD([dict(params=ps, lr=lr) for ps, lr in spec], lr=0.1, **hp)
-    ref = SgdReference(spec, hp)
+    ref = Reference([(ps, dict(lr=lr)) for ps, lr in spec], stock("SGD", **hp))
     run_edges(opt, ref, lays, "sgd", "%s %s" % (hp_id, dtype))
 
 
@@ -413,7 +404,7 @@ def test_adam_at_edge_values(tok_lib, hp_id, dtype):
     spec = [(lays[0].params, 1e-3)]
     opt = getattr(optim, "MasterWeight" + cls)([dict(params=ps, lr=lr) for ps, lr in spec],
                                                lr=1e-3, **hp)
-    ref = AdamReference(spec, cls, hp)
+    ref = Reference([(ps, dict(lr=lr)) for ps, lr in spec], stock(cls, **hp))
     zero_grad = []
 
     def first(params, opt):
@@ -439,7 +430,7 @@ def test_lamb_at_edge_values(tok_lib, dtype):
     import torch
     from torch_on_k8s_b200.optim import MasterWeightLAMB
     dev = torch.device("cuda", 0)
-    dt = _dtype(dtype)
+    dt = harness.torch_dtype(dtype)
     nan_at, inf_at, big_at = NORM_CHUNK + 1234, 500, 7
     decay = Layout(dev, dt, ((2 * NORM_CHUNK + 4000, 0, 0), (1001, 1, 1), (2000, 0, 0), (513, 0, 0),
                              (1000, 0, 0), (4096, 3, 5)), 20)
@@ -447,9 +438,10 @@ def test_lamb_at_edge_values(tok_lib, dtype):
                    masters=MASTER_CATALOGUE, states=STATE_CATALOGUE)
     lays = [decay, plain]
     params, lay_of = flatten(lays)
-    groups = [(decay.params, 1e-3, WD), (plain.params, 5e-4, 0.0)]
-    opt = MasterWeightLAMB([dict(params=ps, lr=lr, weight_decay=wd) for ps, lr, wd in groups])
-    ref = LambReference(groups)
+    groups = [(decay.params, dict(lr=1e-3, weight_decay=WD)),
+              (plain.params, dict(lr=5e-4, weight_decay=0.0))]
+    opt = MasterWeightLAMB([dict(params=ps, **o) for ps, o in groups])
+    ref = Reference(groups, RefLAMB)
     sch = sched(opt)
     gen = torch.Generator(device=dev).manual_seed(6)
     nd = len(decay.params)
@@ -505,17 +497,16 @@ def test_clipped_step_after_nonfinite_norm(tok_lib, case, dtype):
     from torch_on_k8s_b200 import optim
     dev = torch.device("cuda", 0)
     cls, hp = CLIP_CASES[case]
-    lays = [Layout(dev, _dtype(dtype), SEGMENTS[1:], 30)]
+    lays = [Layout(dev, harness.torch_dtype(dtype), SEGMENTS[1:], 30)]
     params, lay_of = flatten(lays)
     if cls == "LAMB":
-        groups = [(params[:3], 1e-3, WD), (params[3:], 1e-3, 0.0)]
-        opt = optim.MasterWeightLAMB([dict(params=ps, lr=lr, weight_decay=wd)
-                                      for ps, lr, wd in groups], max_grad_norm=CLIP)
-        ref = LambReference(groups, clip=CLIP)
+        groups = [(params[:3], dict(lr=1e-3, weight_decay=WD)),
+                  (params[3:], dict(lr=1e-3, weight_decay=0.0))]
+        opt = optim.MasterWeightLAMB([dict(params=ps, **o) for ps, o in groups], max_grad_norm=CLIP)
+        ref = Reference(groups, RefLAMB, clip=CLIP)
     else:
-        spec = [(params, 1e-3)]
         opt = getattr(optim, "MasterWeight" + cls)(params, lr=1e-3, max_grad_norm=CLIP, **hp)
-        ref = ClipReference(spec, cls, hp, CLIP)
+        ref = Reference([(params, dict(lr=1e-3))], stock(cls, **hp), clip=CLIP)
     sch = sched(opt)
     gen = torch.Generator(device=dev).manual_seed(7)
     for step in range(5):
@@ -526,7 +517,7 @@ def test_clipped_step_after_nonfinite_norm(tok_lib, case, dtype):
         total = torch.nn.utils.get_total_norm([g.float() for g in grads])
         opt.step()
         sch.step()
-        ret = ref.step(grads)
+        ret, _ = ref.step(grads)
         if cls != "LAMB":
             total = ret
         where = "%s %s step %d" % (case, dtype, step)
@@ -553,20 +544,20 @@ def test_unscaled_step_at_finite_extremes(tok_lib, case, dtype):
     cls, hp = SCALED_CASES[case]
     finite = tuple(e for e in GRAD_CATALOGUE[dtype] if e[0] not in NONFINITE)
     segs = LAMB_SEGMENTS if cls == "LAMB" else SEGMENTS
-    lays = [Layout(dev, _dtype(dtype), segs, 40 + k, grads=finite) for k in range(2)]
+    lays = [Layout(dev, harness.torch_dtype(dtype), segs, 40 + k, grads=finite) for k in range(2)]
     params, lay_of = flatten(lays)
     if cls == "LAMB":
-        groups = [(lays[0].params, 1e-3, WD), (lays[1].params, 5e-4, 0.0)]
-        opt = optim.MasterWeightLAMB([dict(params=ps, lr=lr, weight_decay=wd)
-                                      for ps, lr, wd in groups], loss_scale=new_loss_scale())
-        scaler = torch.amp.GradScaler("cuda", init_scale=INIT_SCALE, growth_interval=INTERVAL)
-        scaler._lazy_init_scale_growth_tracker(dev)
-        ref = LambReference(groups, scaler=scaler)
+        groups = [(lays[0].params, dict(lr=1e-3, weight_decay=WD)),
+                  (lays[1].params, dict(lr=5e-4, weight_decay=0.0))]
+        opt = optim.MasterWeightLAMB([dict(params=ps, **o) for ps, o in groups],
+                                     loss_scale=new_loss_scale())
+        ref = Reference(groups, RefLAMB, scale=(INIT_SCALE, INTERVAL))
     else:
         spec = [(lays[0].params, 1e-2), (lays[1].params, 5e-4)]
         opt = getattr(optim, "MasterWeight" + cls)([dict(params=ps, lr=lr) for ps, lr in spec],
                                                    lr=1e-2, loss_scale=new_loss_scale(), **hp)
-        ref = ScaledReference(spec, cls, hp, None)
+        ref = Reference([(ps, dict(lr=lr)) for ps, lr in spec], stock(cls, **hp),
+                        scale=(INIT_SCALE, INTERVAL))
     sch = sched(opt)
     gen = torch.Generator(device=dev).manual_seed(8)
     scales = []
@@ -579,11 +570,11 @@ def test_unscaled_step_at_finite_extremes(tok_lib, case, dtype):
         opt.step()
         sch.step()
         where = "%s %s step %d" % (case, dtype, step)
+        total, found = ref.step(grads)
         if cls == "LAMB":
-            found = ref.step(grads)
-            assert not found and same_bits(opt.loss_scale.scale_tensor, ref.scaler._scale), where
+            assert not found.item() and same_bits(opt.loss_scale.scale_tensor, ref.scaler._scale), \
+                where
         else:
-            total, found = ref.step(grads)
             assert not scaling_matches(opt, ref, found, total), where
         assert not opt.step_skipped, where
         assert_matches(opt, params, ref, lay_of, where, step)
@@ -604,18 +595,17 @@ def test_half_write_back_at_range_limits(tok_lib, case, dtype):
     masters = tuple((name, b32) for name, b32, _, _ in WRITE_BACK)
     want = {name: (bf if dtype == "bf16" else h) for name, _, bf, h in WRITE_BACK}
     segs = LAMB_SEGMENTS if case == "lamb" else SEGMENTS
-    lays = [Layout(dev, _dtype(dtype), segs, 50, masters=masters)]
+    lays = [Layout(dev, harness.torch_dtype(dtype), segs, 50, masters=masters)]
     params, lay_of = flatten(lays)
     if case == "lamb":
-        groups = [(params, lr, 0.0)]
         opt = optim.MasterWeightLAMB([dict(params=params, lr=lr, weight_decay=0.0)])
-        ref = LambReference(groups)
+        ref = Reference([(params, dict(lr=lr, weight_decay=0.0))], RefLAMB)
     elif case == "adam":
         opt = optim.MasterWeightAdam(params, lr=lr)
-        ref = AdamReference([(params, lr)], "Adam", {})
+        ref = Reference([(params, dict(lr=lr))], stock("Adam"))
     else:
         opt = optim.MasterWeightSGD(params, lr=lr)
-        ref = SgdReference([(params, lr)], {})
+        ref = Reference([(params, dict(lr=lr))], stock("SGD"))
     sch = sched(opt)
     gen = torch.Generator(device=dev).manual_seed(9)
     written = None

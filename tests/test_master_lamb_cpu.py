@@ -2,21 +2,21 @@
 torch.optim.Adam's messages where Adam rejects the same), its defaults, fp32 state and a CPU float32
 `step` across state_dict, and the segment table built from real DDP gradient buckets."""
 import ctypes
-import os
-import tempfile
 
 import pytest
 import torch
 import torch.nn as nn
 
+import master_weight
+
+# tok_lamb_master_step arguments with fake (never dereferenced) table and scratch pointers
+ARGS = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=1, lr=1e-3, beta1=0.9,
+            beta2=0.999, eps=1e-6, weight_decay=1e-2, step=1.0, partials=ctypes.c_void_p(512),
+            inv_scale=None, grad_coef=None, stream=None)
+
 
 def _args(**over):
-    """tok_lamb_master_step arguments with fake (never dereferenced) table and scratch pointers."""
-    a = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=1, lr=1e-3, beta1=0.9,
-             beta2=0.999, eps=1e-6, weight_decay=1e-2, step=1.0, partials=ctypes.c_void_p(512),
-             inv_scale=None, grad_coef=None, stream=None)
-    a.update(over)
-    return list(a.values())
+    return master_weight.abi_args(ARGS, **over)
 
 
 NAN, INF = float("nan"), float("inf")
@@ -36,23 +36,15 @@ NAN, INF = float("nan"), float("inf")
     (dict(step=0.0), "step"), (dict(step=0.5), "step"), (dict(step=NAN), "step"),
     (dict(step=INF), "step"), (dict(partials=None), "null partials")])
 def test_abi_rejects_bad_arguments(tok_lib, bad, says):
-    from torch_on_k8s_b200 import _ffi
-    assert tok_lib.tok_lamb_master_step(*_args(**bad)) == _ffi.TOK_ERR_INVALID
-    msg = _ffi.last_error()
-    assert "tok_lamb_master_step" in msg and says in msg, msg
+    master_weight.refused(tok_lib, "tok_lamb_master_step", _args(**bad), says)
 
 
 def test_abi_needs_a_gpu(tok_lib):
-    if torch.cuda.is_available():
-        pytest.skip("box has a GPU")
-    from torch_on_k8s_b200 import _ffi
     fake = ctypes.c_void_p(1024)
-    for ok in (_args(), _args(dtype=2, weight_decay=0.0), _args(inv_scale=fake),
-               _args(inv_scale=fake, grad_coef=fake), _args(grad_coef=fake),
-               _args(beta1=0.0, beta2=0.0, eps=0.0, lr=0.0, step=1e6),
-               _args(chunks=0, partials=None)):
-        assert tok_lib.tok_lamb_master_step(*ok) == _ffi.TOK_ERR_NO_DEVICE
-        assert "no CPU fallback" in _ffi.last_error()
+    master_weight.needs_a_gpu([(tok_lib.tok_lamb_master_step, a) for a in (
+        _args(), _args(dtype=2, weight_decay=0.0), _args(inv_scale=fake),
+        _args(inv_scale=fake, grad_coef=fake), _args(grad_coef=fake),
+        _args(beta1=0.0, beta2=0.0, eps=0.0, lr=0.0, step=1e6), _args(chunks=0, partials=None))])
 
 
 def _bf16_param():
@@ -169,64 +161,19 @@ def test_segment_table_matches_ddp_bucket_views():
     .gradients() point, parameter by parameter, at the gradient views inside the bucket and at the
     parameter's master and moments, with chunks of TOK_NORM_CHUNK elements, before and after DDP's
     bucket rebuild."""
-    import torch.distributed as dist
-    from torch.nn.parallel import DistributedDataParallel as DDP
     from torch_on_k8s_b200.optim import NORM_CHUNK, MasterWeightLAMB, segment_table
-
-    torch.manual_seed(0)
-    model = nn.Sequential(nn.Conv2d(3, 24, 3, bias=False), nn.BatchNorm2d(24), nn.ReLU(),
-                          nn.Conv2d(24, 37, 3), nn.Flatten(), nn.Linear(37 * 4 * 4, 1001),
-                          nn.Linear(1001, 70)).to(torch.bfloat16).to(memory_format=torch.channels_last)
+    keys = ("master_param", "exp_avg", "exp_avg_sq")
+    model = master_weight.ddp_table_model(70)
     opt = MasterWeightLAMB(model.parameters())
     for p in model.parameters():
         st = opt.state[p]
-        for k in ("exp_avg", "exp_avg_sq"):
+        for k in keys[1:]:
             st[k] = torch.zeros_like(st["master_param"], memory_format=torch.preserve_format)
-    seen = []
-
-    def hook(state, bucket):
-        buf = bucket.buffer()
-        esz = buf.element_size()
-        sts = [opt.state[p] for p in bucket.parameters()]
-        entries = [(g, p, st["master_param"], st["exp_avg"], st["exp_avg_sq"])
-                   for p, g, st in zip(bucket.parameters(), bucket.gradients(), sts)]
-        rows, chunks = segment_table(entries, NORM_CHUNK)
-        want = [((g.data_ptr() - buf.data_ptr()) // esz, g.numel(), p.data_ptr(),
-                 tuple(st[k].data_ptr() for k in ("master_param", "exp_avg", "exp_avg_sq")))
-                for p, g, st in zip(bucket.parameters(), bucket.gradients(), sts)]
-        seen.append((bucket.index(), buf.data_ptr(), esz, buf.numel(), rows, chunks, want))
-        fut = torch.futures.Future()
-        fut.set_result(buf)
-        return fut
-
-    with tempfile.TemporaryDirectory() as tmp:
-        dist.init_process_group("gloo", init_method="file://" + os.path.join(tmp, "store"), rank=0,
-                                world_size=1)
-        try:
-            ddp = DDP(model, bucket_cap_mb=0.25, gradient_as_bucket_view=True)
-            ddp.register_comm_hook(None, hook)
-            for step in range(2):
-                x = torch.randn(2, 3, 8, 8).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
-                ddp(x).float().sum().backward()
-                seen.append(("step", step))
-        finally:
-            dist.destroy_process_group()
-    layouts, step_of, multi = {}, 0, False
-    for rec in seen:
-        if rec[0] == "step":
-            step_of += 1
-            continue
-        index, base, esz, numel, rows, chunks, want = rec
-        assert len(rows) == len(want) > 0
-        chunk = covered = 0
-        for row, (off, n, pp, state) in zip(rows, want):
-            assert len(row) == 7   # tok_lamb_segment_t: grad, param, 3 fp32 arrays, numel, chunk0
-            assert row[0] == base + off * esz and row[1] == pp and row[2:5] == state
-            assert row[5] == n and row[6] == chunk and 0 <= off and off + n <= numel
-            chunk += -(-n // NORM_CHUNK)
-            multi |= n > NORM_CHUNK
-            covered += n
-        assert chunks == chunk and covered == numel
-        layouts.setdefault(step_of, []).append((index, tuple(r[0] for r in rows)))
-    assert multi   # a parameter spans several chunks
-    assert sorted(layouts) == [0, 1] and len(layouts[1]) >= 2 and layouts[0] != layouts[1], layouts
+    # tok_lamb_segment_t: grad, param, 3 fp32 arrays, numel, chunk0
+    buckets = master_weight.check_tables_match_ddp_buckets(
+        model, lambda pairs: segment_table([(g, p) + tuple(opt.state[p][k] for k in keys)
+                                            for p, g in pairs], NORM_CHUNK),
+        lambda p, g, chunk0: (g.data_ptr(), p.data_ptr(),
+                              *(opt.state[p][k].data_ptr() for k in keys), g.numel(), chunk0),
+        NORM_CHUNK)
+    assert any(n > NORM_CHUNK for views in buckets for _, _, n in views)   # several chunks

@@ -31,115 +31,17 @@ sign of zero included:
   * ElasticDataParallel.reduce_grads(optimizer=...) across a 2 -> 3 -> 2 re-form schedule with
     hand_over: a joiner holds the root's masters and momenta, and replicas stay identical.
 """
-import hashlib
-
-import numpy as np
 import pytest
 
 import harness
-from test_master_sgd_gpu import bits, make_bf16, ragged, same_bits, sched
-from test_training_paths_gpu import devices_for, free_port, make_batch, make_model
+from master_weight import INIT_SCALE, INTERVAL, LARS_LR as LR, RefLARS, Reference, check_against, \
+    check_hand_over, ddp_replica, elastic_replica, fill_grads, make_bf16, new_loss_scale, ragged, \
+    same_bits, sched
+from test_training_paths_gpu import devices_for, free_port
 
 pytestmark = pytest.mark.gpu
 
 STEPS = 4
-LR = 0.1   # the scheduler takes it to 0.03 and 0.009: none a power of two
-DEFAULTS = dict(lr=LR, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False,
-                trust_coefficient=0.02, clip=True, eps=1e-8, lars=True)
-
-
-def _lars_optimizer_class():
-    import torch
-    from torch.optim.sgd import sgd
-
-    class RefLARS(torch.optim.Optimizer):
-        """The restatement in the module docstring, as a torch optimizer (so that an LR scheduler and
-        GradScaler drive it as they drive MasterWeightLARS)."""
-
-        def __init__(self, params):
-            super().__init__(params, dict(DEFAULTS))
-
-        @torch.no_grad()
-        def step(self, closure=None):
-            for group in self.param_groups:
-                W = [w for w in group["params"] if w.grad is not None]
-                if not W:
-                    continue
-                G = [w.grad for w in W]
-                lr, wd = group["lr"], group["weight_decay"]
-                if group["lars"]:
-                    wn, gn = torch._foreach_norm(W), torch._foreach_norm(G)
-                    for w, g, a, b in zip(W, G, wn, gn):
-                        r = group["trust_coefficient"] * a / (b + a * wd + group["eps"])
-                        if group["clip"]:
-                            r = torch.clamp(r / lr, max=1.0)
-                        g.copy_(torch.where((a != 0) & (b != 0), (g + wd * w) * r, g))
-                    wd = 0.0
-                bufs = [self.state[w].get("momentum_buffer") for w in W]
-                sgd(W, G, bufs, foreach=True, weight_decay=wd, momentum=group["momentum"], lr=lr,
-                    dampening=group["dampening"], nesterov=group["nesterov"], maximize=False)
-                if group["momentum"] != 0:
-                    for w, b in zip(W, bufs):
-                        self.state[w]["momentum_buffer"] = b
-
-    return RefLARS
-
-
-class Reference:
-    """RefLARS on fp32 copies of the parameters, then P.copy_(W); optionally behind GradScaler and
-    clip_grad_norm_, as the stock loop stores master.grad."""
-
-    def __init__(self, groups, masters=None, clip=None, scaler=None):
-        """groups: [(params, group options)]"""
-        import torch
-        params = [p for ps, _ in groups for p in ps]
-        self.params = [p.detach().clone(memory_format=torch.preserve_format) for p in params]
-        self.masters = [w.detach().clone(memory_format=torch.preserve_format) for w in masters] \
-            if masters is not None else \
-            [p.detach().to(torch.float32, memory_format=torch.preserve_format) for p in params]
-        spec, k = [], 0
-        for ps, kw in groups:
-            spec.append(dict(params=self.masters[k:k + len(ps)], **kw))
-            k += len(ps)
-        self.opt = _lars_optimizer_class()(spec)
-        self.sched = sched(self.opt)
-        self.clip, self.scaler = clip, scaler
-
-    def step(self, grads):
-        import torch
-        for w, g in zip(self.masters, grads):
-            w.grad = None if g is None else g.to(torch.float32, memory_format=torch.preserve_format)
-        found = None
-        if self.scaler is not None:
-            self.scaler.unscale_(self.opt)
-        if self.clip is not None:
-            torch.nn.utils.clip_grad_norm_(self.masters, self.clip)
-        if self.scaler is not None:
-            found = sum(v for v in self.scaler._found_inf_per_device(self.opt).values()).item()
-            self.scaler.step(self.opt)
-            self.scaler.update()
-        else:
-            self.opt.step()
-        self.sched.step()
-        if not found:
-            with torch.no_grad():
-                for p, w in zip(self.params, self.masters):
-                    p.copy_(w)
-        return found
-
-
-def check_against(opt, params, ref, where):
-    bad = []
-    for i, p in enumerate(params):
-        st, rst = opt.state[p], ref.opt.state.get(ref.masters[i], {})
-        if not same_bits(st["master_param"], ref.masters[i]):
-            bad.append((i, "master"))
-        if not same_bits(p, ref.params[i]):
-            bad.append((i, "param"))
-        a, b = st.get("momentum_buffer"), rst.get("momentum_buffer")
-        if (a is None) != (b is None) or (a is not None and not same_bits(a, b)):
-            bad.append((i, "momentum_buffer"))
-    assert not bad, "%s: %d tensors differ from the reference, first %s" % (where, len(bad), bad[:5])
 
 
 def new_opt(groups, **kw):
@@ -148,42 +50,17 @@ def new_opt(groups, **kw):
     return MasterWeightLARS([dict(params=ps, **o) for ps, o in groups], lr=LR, **kw)
 
 
-def fill(grads_of, dev, gen, scale=1.0):
-    """Fresh gradients for [(params, views)]: views None gives each parameter its own, else
-    (flat gradient buffer, element offsets)."""
-    import torch
-    grads = []
-    for ps, views in grads_of:
-        if views is None:
-            for p in ps:
-                p.grad = torch.empty_like(p).copy_(
-                    torch.randn(p.shape, device=dev, generator=gen) * 1e-2 * scale)
-                grads.append(p.grad)
-        else:
-            gflat, goffs = views
-            gflat.copy_(torch.randn(gflat.shape, device=dev, generator=gen) * 1e-2 * scale)
-            for p, o in zip(ps, goffs):
-                p.grad = gflat[o:o + p.numel()].view(p.shape)
-                grads.append(p.grad)
-    return grads
-
-
-def _dtype(name):
-    import torch
-    return {"bf16": torch.bfloat16, "f16": torch.float16}[name]
-
-
 def run(groups, views, dev, steps=STEPS, seed=1, late=None, where=""):
     """Step MasterWeightLARS and the reference side by side and compare after every step; `late`
     misses its gradient at step 1."""
     import torch
     params = [p for ps, _ in groups for p in ps]
     opt = new_opt(groups)
-    ref = Reference(groups)
+    ref = Reference(groups, RefLARS)
     sch = sched(opt)
     gen = torch.Generator(device=dev).manual_seed(seed)
     for step in range(steps):
-        grads = fill(views, dev, gen)
+        grads = fill_grads(views, dev, gen)
         if late is not None and step == 1:
             params[late].grad = None
             grads[late] = None
@@ -211,7 +88,7 @@ def test_standalone_matches_reference(tok_lib, kind, dtype, config):
     import torch
     from torch_on_k8s_b200.optim import lars_param_groups
     dev = torch.device("cuda", 0)
-    t = _dtype(dtype)
+    t = harness.torch_dtype(dtype)
     kw = CONFIGS[config]
     sgd_kw = {k: v for k, v in kw.items() if k in ("momentum", "dampening", "nesterov")}
     if kind == "resnet50":
@@ -251,7 +128,7 @@ def test_thousands_of_trust_ratios(tok_lib, clip):
           for n, e in zip(sizes, wexp)]
     groups = [(ps, dict(momentum=0.9, weight_decay=1e-3, clip=clip))]
     opt = new_opt(groups)
-    ref = Reference(groups)
+    ref = Reference(groups, RefLARS)
     sch = sched(opt)
     for step in range(3):
         grads = []
@@ -275,7 +152,7 @@ def test_more_partials_than_cleanup_threads(tok_lib, dtype):
     """Two tensors of more than 512 chunks, one of each accumulator mapping, and a small one."""
     import torch
     dev = torch.device("cuda", 0)
-    t = _dtype(dtype)
+    t = harness.torch_dtype(dtype)
     g = torch.Generator(device=dev).manual_seed(3)
     big = 512 * 65536
     ps = [torch.nn.Parameter((torch.randn(big + 4 * 1001, device=dev, generator=g) * 0.1).to(t)),
@@ -299,10 +176,10 @@ def test_zero_norms_and_zero_lr(tok_lib):
               (frozen, dict(momentum=0.9, weight_decay=1e-2, lr=0.0))]
     params = decay + frozen
     opt = new_opt(groups)
-    ref = Reference(groups)
+    ref = Reference(groups, RefLARS)
     sch = sched(opt)
     for step in range(3):
-        grads = fill([(params, None)], dev, g)
+        grads = fill_grads([(params, None)], dev, g)
         if step == 0:   # decay[1] (zero master) and decay[2] get zero gradients
             for i in (1, 2):
                 grads[i].zero_()
@@ -328,7 +205,7 @@ def test_ieee_edges(tok_lib, dtype, clip):
     path); and a group whose decay term overflows (a * wd = inf, so r = 0)."""
     import torch
     dev = torch.device("cuda", 0)
-    t = _dtype(dtype)
+    t = harness.torch_dtype(dtype)
     tiny = float(torch.finfo(t).tiny)
     edge = {"inf": [float("inf"), -float("inf")], "nan": [float("nan")],
             "zero": [0.0, -0.0], "sub": [tiny / 4, -tiny / 2, tiny * 0.75]}
@@ -363,7 +240,7 @@ def test_ieee_edges(tok_lib, dtype, clip):
     opt = new_opt(groups)
     for p, w in zip(ps, masters):
         opt.state[p]["master_param"].copy_(w)
-    ref = Reference(groups, masters=[opt.state[p]["master_param"] for p in params])
+    ref = Reference(groups, RefLARS, masters=[opt.state[p]["master_param"] for p in params])
     sch = sched(opt)
     for step in range(3):
         gflat.copy_(torch.randn(gflat.shape, device=dev, generator=g) * 1e-2)
@@ -393,9 +270,9 @@ def test_ieee_edges(tok_lib, dtype, clip):
                          ids=["clipped", "scaled", "clipped_scaled"])
 def test_clipping_and_loss_scaling(tok_lib, dtype, clip, scaled):
     import torch
-    from torch_on_k8s_b200.optim import DynamicLossScale, lars_param_groups
+    from torch_on_k8s_b200.optim import lars_param_groups
     dev = torch.device("cuda", 0)
-    t = _dtype(dtype)
+    t = harness.torch_dtype(dtype)
     lg = lars_param_groups(make_bf16(0, dev).to(t).parameters(), 1e-4)
     ps, gflat, goffs = ragged(dev, t)
     groups = [(lg[0]["params"], dict(momentum=0.9, weight_decay=1e-4)),
@@ -403,19 +280,14 @@ def test_clipping_and_loss_scaling(tok_lib, dtype, clip, scaled):
               (ps, dict(momentum=0.9, weight_decay=1e-3, clip=False))]
     views = [(lg[0]["params"] + lg[1]["params"], None), (ps, (gflat, goffs))]
     params = [p for gr in groups for p in gr[0]]
-    init_scale, interval = 3.0 * 2.0 ** 12, 3   # not a power of two: unscale and clip round twice
-    ls = DynamicLossScale(init_scale=init_scale, growth_interval=interval) if scaled else None
+    ls = new_loss_scale() if scaled else None
     opt = new_opt(groups, max_grad_norm=clip, loss_scale=ls)
-    scaler = None
-    if scaled:
-        scaler = torch.amp.GradScaler("cuda", init_scale=init_scale, growth_interval=interval)
-        scaler._lazy_init_scale_growth_tracker(dev)
-    ref = Reference(groups, clip=clip, scaler=scaler)
+    ref = Reference(groups, RefLARS, clip=clip, scale=(INIT_SCALE, INTERVAL) if scaled else None)
     sch = sched(opt)
     gen = torch.Generator(device=dev).manual_seed(31)
     late, overflow, skipped = 1, 3, []
     for it in range(7):
-        grads = fill(views, dev, gen, ls.get_scale() if scaled else 1.0)
+        grads = fill_grads(views, dev, gen, ls.get_scale() if scaled else 1.0)
         if it < 4:   # its first step is the skipped one: it must create no state
             params[late].grad = None
             grads[late] = None
@@ -423,11 +295,12 @@ def test_clipping_and_loss_scaling(tok_lib, dtype, clip, scaled):
             grads[-1].view(-1)[it] = float("inf")
         opt.step()
         sch.step()
-        found = ref.step(grads)
+        _, found = ref.step(grads)
         torch.cuda.synchronize()
         check_against(opt, params, ref, "%s %s %s iteration %d" % (dtype, clip, scaled, it))
         if scaled:
-            assert same_bits(ls.scale_tensor, scaler._scale) and opt.step_skipped == bool(found)
+            assert same_bits(ls.scale_tensor, ref.scaler._scale) and \
+                opt.step_skipped == bool(found.item())
             skipped.append(opt.step_skipped)
         if scaled and it == overflow:
             assert "momentum_buffer" not in opt.state[params[late]]
@@ -454,7 +327,7 @@ def test_is_larc_within_norm_tolerance(tok_lib):
     larc_sgd = torch.optim.SGD(W, lr=LR, momentum=0.9, weight_decay=0.0)
     gen = torch.Generator(device=dev).manual_seed(2)
     for step in range(3):
-        grads = fill([(params, None)], dev, gen)
+        grads = fill_grads([(params, None)], dev, gen)
         opt.step()
         with torch.no_grad():   # apex.parallel.LARC.step, clip=True
             for w, gr in zip(W, grads):
@@ -476,192 +349,27 @@ def test_is_larc_within_norm_tolerance(tok_lib):
 
 
 # ---- DDP through Replica.wrap -------------------------------------------------------------------
-DDP_STEPS = 4
 WD = 1e-3
-
-
-def state_digests(opt, params):
-    return [hashlib.sha1(bits(t).cpu().numpy().tobytes()).hexdigest() if t is not None else None
-            for p in params for t in (p, opt.state[p].get("master_param"),
-                                      opt.state[p].get("momentum_buffer"))]
-
-
-def ddp_lars_replica(rank, world, device, path, cases, job):
-    import os
-    import torch
-    import torch.distributed as dist
-    from oracle.allreduce_oracle import allreduce_oracle
-    from torch_on_k8s_b200 import ddp_hook
-    from torch_on_k8s_b200.optim import MasterWeightLARS, lars_param_groups
-    from torch_on_k8s_b200.worker import init_replica
-
-    spec = cases[0]
-    os.environ.update(RANK=str(rank), WORLD_SIZE=str(world), TOK8S_RDZV=path)
-    torch.cuda.set_device(device)
-    dev = torch.device("cuda", device)
-    dist.init_process_group("gloo", init_method="tcp://127.0.0.1:%d" % spec["port"], rank=rank,
-                            world_size=world)
-    rep = init_replica(job, device=device, bootstrap_backend="gloo")
-    model = make_model("conv", 1000 + rank, dev)       # every replica starts different
-    groups = lars_param_groups(model.parameters(), WD)
-    params = [p for g in groups for p in g["params"]]  # in the optimizer's order
-    pidx = {p.data_ptr(): i for i, p in enumerate(params)}
-    opt = MasterWeightLARS(groups, lr=LR, momentum=0.9)
-    sch = sched(opt)
-    buckets = []
-    real_call = ddp_hook.BucketAllreduceHook.__call__
-
-    def traced(self, state, bucket):
-        buf = bucket.buffer()
-        pre = buf.clone()     # on the compute stream, before the exchange may touch the bucket
-        esz = buf.element_size()
-        views = [(pidx[p.data_ptr()], (g.data_ptr() - buf.data_ptr()) // esz, g.numel())
-                 for p, g in zip(bucket.parameters(), bucket.gradients())]
-        buckets.append(dict(step=step_no[0], pre=pre, views=views))
-        return real_call(self, state, bucket)
-    ddp_hook.BucketAllreduceHook.__call__ = traced
-    step_no = [0]
-    try:
-        ddp, hook = rep.wrap(model, bucket_cap_mb=1, optimizer=opt)
-        torch.cuda.synchronize()
-        init_p = [p.detach().clone(memory_format=torch.preserve_format) for p in params]
-        init_w = [opt.state[p]["master_param"].clone(memory_format=torch.preserve_format)
-                  for p in params]
-        for step in range(DDP_STEPS):
-            step_no[0] = step
-            x, y = make_batch("conv", rank, step, dev)
-            opt.zero_grad(set_to_none=False)
-            torch.nn.functional.cross_entropy(ddp(x).float(), y).backward()
-            opt.step()
-            sch.step()
-            torch.cuda.synchronize()
-            rep.comm.status()
-        stepped_in_buckets = len(opt._stepped) == 0 and any(k[0] == "bucket" for k in opt._tables) \
-            and not any(k[0] == "group" for k in opt._tables)
-        mine = [dict(step=b["step"], views=b["views"], pre=harness.from_torch(b["pre"], "bf16"))
-                for b in buckets]
-        everyone = [None] * world
-        dist.all_gather_object(everyone, mine)
-        n_lars = len(groups[0]["params"])
-        ref = Reference([(init_p[:n_lars], dict(momentum=0.9, weight_decay=WD)),
-                         (init_p[n_lars:], dict(momentum=0.9, lars=False))], masters=init_w)
-        for step in range(DDP_STEPS):
-            slices = {}
-            for r in range(world):
-                for b in everyone[r]:
-                    if b["step"] == step:
-                        for pi, off, n in b["views"]:
-                            slices.setdefault(pi, [None] * world)[r] = b["pre"][off:off + n]
-            assert sorted(slices) == list(range(len(params))), (step, sorted(slices))
-            grads = []
-            for pi, p in enumerate(params):
-                avg = allreduce_oracle(slices[pi], "bf16", "bf16", "bf16", 1.0 / world)
-                g = torch.empty_strided(p.shape, p.stride(), dtype=torch.bfloat16, device=dev)
-                g.as_strided((p.numel(),), (1,)).copy_(
-                    torch.from_numpy(avg.view(np.int16).copy()).view(torch.bfloat16))
-                grads.append(g)
-            ref.step(grads)
-        torch.cuda.synchronize()
-        check_against(opt, params, ref, "rank %d of %d" % (rank, world))
-        layouts = {tuple(v for v in b["views"]) for b in buckets}
-        return dict(state=state_digests(opt, params), in_buckets=stepped_in_buckets,
-                    layouts=len(layouts))
-    finally:
-        ddp_hook.BucketAllreduceHook.__call__ = real_call
-        rep.close()
 
 
 @pytest.mark.parametrize("world", [1, 2, 3])
 def test_ddp_hook_step_matches_reference(tok_lib, n_gpus, world):
     devs, env = devices_for(world, n_gpus)
-    res = harness.launch(world, [dict(port=free_port())], devices=devs, mode="proc", env=env,
-                         job="mlars%d" % world, body=ddp_lars_replica, timeout=600)
+    case = dict(port=free_port(), opt="LARS", kw=dict(lr=LR, momentum=0.9), param_groups=(WD,),
+                ref_groups=[dict(momentum=0.9, weight_decay=WD), dict(momentum=0.9, lars=False)],
+                dtype="bf16", sched=True, steps=4, keys=("momentum_buffer",))
+    res = harness.launch(world, [case], devices=devs, mode="proc", env=env, job="mlars%d" % world,
+                         body=ddp_replica, timeout=600)
     for r in range(world):
         assert res[r]["in_buckets"], "rank %d: a step was not taken behind its bucket" % r
         assert res[r]["state"] == res[0]["state"], "rank %d's state differs from rank 0's" % r
 
 
 # ---- ElasticDataParallel --------------------------------------------------------------------------
-def elastic_lars_replica(proc, world, device, path, cases, job):
-    """Processes 0 and 1 train at world 2; process 2 joins at epoch 1 (world 3); process 1 leaves at
-    epoch 2 and process 2 becomes rank 1."""
-    import torch
-    from torch_on_k8s_b200.comm import Communicator
-    from torch_on_k8s_b200.elastic_dp import ElasticDataParallel
-    from torch_on_k8s_b200.optim import MasterWeightLARS, lars_param_groups
-
-    torch.cuda.set_device(device)
-    dev = torch.device("cuda", device)
-    joiner = proc == 2
-    model = make_bf16(99 if joiner else 0, dev)
-    if joiner:
-        comm = Communicator(job, 2, 3, device, rendezvous_path=path, max_world=3, epoch=1)
-    else:
-        comm = Communicator(job, proc, 2, device, rendezvous_path=path, max_world=3)
-    edp = ElasticDataParallel(model, comm, bucket_cap_mb=1)
-    opt = MasterWeightLARS(lars_param_groups(model.parameters()), lr=LR, momentum=0.9)
-    params = [p for g in opt.param_groups for p in g["params"]]
-    out = dict(proc=proc, buckets=len(edp.buckets), steps=[], handovers=[])
-
-    def train(phase, n):
-        for s in range(n):
-            edp.zero_grad()
-            g = torch.Generator().manual_seed(1000 * phase + 10 * s + proc)
-            x = torch.randn(32, 64, generator=g).to(dev).to(torch.bfloat16)
-            y = torch.randint(0, 10, (32,), generator=g).to(dev)
-            torch.nn.functional.cross_entropy(edp(x).float(), y).backward()
-            edp.reduce_grads(optimizer=opt)
-            opt.step()
-            torch.cuda.synchronize()
-            comm.status()
-            out["steps"].append(dict(phase=phase, step=s, rank=comm.rank,
-                                     state=state_digests(opt, params)))
-
-    def hand_over(phase):
-        before = state_digests(opt, params)
-        edp.hand_over(opt, 0)
-        comm.status()
-        out["handovers"].append(dict(phase=phase, rank=comm.rank, before=before,
-                                     after=state_digests(opt, params)))
-
-    try:
-        if not joiner:
-            train(0, 2)
-            edp.reform(3, proc, 0b11, 1)
-        hand_over(1)
-        train(1, 2)
-        if proc == 1:
-            return out
-        edp.reform(2, 0 if proc == 0 else 1, 0b101, 2)
-        hand_over(2)
-        train(2, 2)
-    finally:
-        comm.close()
-    return out
-
-
 def test_elastic_reforms_hand_over_masters_and_momenta(tok_lib, n_gpus):
     devs, env = devices_for(3, n_gpus)
-    res = harness.launch(3, [{}], devices=devs, mode="proc", env=env, job="mlars-edp",
-                         body=elastic_lars_replica, timeout=600)
-    members = {0: [0, 1], 1: [0, 1, 2], 2: [0, 2]}
-    width = 3   # param, master, momentum_buffer
-    assert res[0]["buckets"] >= 2
-    for phase in (1, 2):
-        procs = members[phase]
-        hos = {p: [h for h in res[p]["handovers"] if h["phase"] == phase][0] for p in procs}
-        root = [p for p in procs if hos[p]["rank"] == 0][0]
-        assert hos[root]["after"] == hos[root]["before"], phase
-        for p in procs:
-            diff = [i for i, (a, b) in enumerate(zip(hos[p]["after"], hos[root]["after"])) if a != b]
-            assert not diff, "phase %d: process %d does not hold the root's parameters, masters " \
-                "and momenta after the hand-over (tensors %s)" % (phase, p, diff)
-    joined = [h for h in res[2]["handovers"] if h["phase"] == 1][0]
-    assert joined["before"][1::width] != joined["after"][1::width]   # the joiner's masters replaced
-    assert joined["before"][2::width] == [None] * len(joined["before"][2::width])
-    assert None not in joined["after"][2::width]   # it had no momenta, and now holds the root's
-    for phase, procs in members.items():
-        for s in range(2):
-            recs = [[x for x in res[p]["steps"] if x["phase"] == phase and x["step"] == s][0]
-                    for p in procs]
-            assert all(r["state"] == recs[0]["state"] for r in recs), (phase, s)
+    case = dict(opt="LARS", kw=dict(lr=LR, momentum=0.9), param_groups=(), dtype="bf16",
+                steps=(2, 2, 2), keys=("momentum_buffer",))
+    res = harness.launch(3, [case], devices=devs, mode="proc", env=env, job="mlars-edp",
+                         body=elastic_replica, timeout=600)
+    check_hand_over(res, 3, fresh=(2,))   # param, master, momentum_buffer: it had no momenta yet

@@ -1,20 +1,20 @@
 """MasterWeightSGD without a GPU: the C ABI's argument checks, what the Python optimizer rejects,
 fp32 state across state_dict, and the segment table built from real DDP gradient buckets."""
 import ctypes
-import os
-import tempfile
 
 import pytest
 import torch
 import torch.nn as nn
 
+import master_weight
+
+# tok_sgd_master_step arguments with a fake (never dereferenced) table pointer
+ARGS = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=1, lr=0.1, momentum=0.9,
+            dampening=0.0, weight_decay=1e-4, nesterov=0, fresh=0, stream=None)
+
 
 def _args(**over):
-    """tok_sgd_master_step arguments with a fake (never dereferenced) table pointer."""
-    a = dict(segments=ctypes.c_void_p(256), count=3, chunks=5, dtype=1, lr=0.1, momentum=0.9,
-             dampening=0.0, weight_decay=1e-4, nesterov=0, fresh=0, stream=None)
-    a.update(over)
-    return list(a.values())
+    return master_weight.abi_args(ARGS, **over)
 
 
 @pytest.mark.parametrize("bad", [
@@ -23,18 +23,12 @@ def _args(**over):
     dict(momentum=-0.5), dict(weight_decay=-1e-4), dict(dampening=float("nan")),
     dict(nesterov=1, momentum=0.0), dict(nesterov=1, dampening=0.1)])
 def test_abi_rejects_bad_arguments(tok_lib, bad):
-    from torch_on_k8s_b200 import _ffi
-    assert tok_lib.tok_sgd_master_step(*_args(**bad)) == _ffi.TOK_ERR_INVALID
-    assert "tok_sgd_master_step" in _ffi.last_error()
+    master_weight.refused(tok_lib, "tok_sgd_master_step", _args(**bad))
 
 
 def test_abi_needs_a_gpu(tok_lib):
-    if torch.cuda.is_available():
-        pytest.skip("box has a GPU")
-    from torch_on_k8s_b200 import _ffi
-    for ok in (_args(), _args(dtype=2, nesterov=1, dampening=0.0, fresh=1), _args(momentum=0.0)):
-        assert tok_lib.tok_sgd_master_step(*ok) == _ffi.TOK_ERR_NO_DEVICE
-        assert "no CPU fallback" in _ffi.last_error()
+    master_weight.needs_a_gpu([(tok_lib.tok_sgd_master_step, a) for a in (
+        _args(), _args(dtype=2, nesterov=1, dampening=0.0, fresh=1), _args(momentum=0.0))])
 
 
 @pytest.mark.parametrize("kw", [dict(lr=-1.0), dict(momentum=-0.1), dict(weight_decay=-1.0),
@@ -95,67 +89,15 @@ def test_masters_and_state_dict_stay_fp32():
 
 def test_segment_table_matches_ddp_bucket_views():
     """A gloo DDP run on the CPU: the table rows built from GradBucket.parameters() / .gradients()
-    point, parameter by parameter, at the gradient views inside the bucket, before and after DDP's
-    bucket rebuild."""
-    import torch.distributed as dist
-    from torch.nn.parallel import DistributedDataParallel as DDP
+    point, parameter by parameter, at the gradient views inside the bucket and at the parameter's
+    master, before and after DDP's bucket rebuild."""
     from torch_on_k8s_b200.optim import CHUNK, MasterWeightSGD, segment_table
-
-    torch.manual_seed(0)
-    model = nn.Sequential(nn.Conv2d(3, 24, 3, bias=False), nn.BatchNorm2d(24), nn.ReLU(),
-                          nn.Conv2d(24, 37, 3), nn.Flatten(), nn.Linear(37 * 4 * 4, 1001),
-                          nn.Linear(1001, 7)).to(torch.bfloat16).to(memory_format=torch.channels_last)
+    model = master_weight.ddp_table_model(7)
     opt = MasterWeightSGD(model.parameters(), lr=0.1, momentum=0.9)
-    seen = []
-
-    def hook(state, bucket):
-        buf = bucket.buffer()
-        esz = buf.element_size()
-        entries = [(g, p, opt.state[p]["master_param"], None)
-                   for p, g in zip(bucket.parameters(), bucket.gradients())]
-        rows, chunks = segment_table(entries)
-        views = []
-        for p, g in zip(bucket.parameters(), bucket.gradients()):
-            assert p.grad is None or p.grad.data_ptr() == g.data_ptr()
-            views.append(((g.data_ptr() - buf.data_ptr()) // esz, g.numel(), p.data_ptr(),
-                          opt.state[p]["master_param"].data_ptr()))
-        seen.append((bucket.index(), buf.data_ptr(), esz, buf.numel(), rows, chunks, views))
-        fut = torch.futures.Future()
-        fut.set_result(buf)
-        return fut
-
-    with tempfile.TemporaryDirectory() as tmp:
-        dist.init_process_group("gloo", init_method="file://" + os.path.join(tmp, "store"), rank=0,
-                                world_size=1)
-        try:
-            ddp = DDP(model, bucket_cap_mb=0.25, gradient_as_bucket_view=True)
-            ddp.register_comm_hook(None, hook)
-            for step in range(2):
-                x = torch.randn(2, 3, 8, 8).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
-                ddp(x).float().sum().backward()
-                seen.append(("step", step))
-        finally:
-            dist.destroy_process_group()
-    layouts = {}
-    step_of = 0
-    offsets = []
-    for rec in seen:
-        if rec[0] == "step":
-            step_of += 1
-            continue
-        index, base, esz, numel, rows, chunks, views = rec
-        offsets += [v[0] for v in views]
-        covered = 0
-        assert len(rows) == len(views) > 0
-        chunk = 0
-        for (g, p, w, m, n, c0), (off, vn, pp, wp) in zip(rows, views):
-            assert g == base + off * esz and n == vn and p == pp and w == wp and m == 0
-            assert 0 <= off and off + n <= numel
-            assert c0 == chunk
-            chunk += -(-n // CHUNK)
-            covered += n
-        assert chunks == chunk and covered == numel   # DDP packs the views without padding
-        layouts.setdefault(step_of, []).append((index, tuple(r[0] for r in rows)))
-    # the rebuild after the first iteration gives a new layout (first bucket 1 MiB, then 0.25 MiB)
-    assert sorted(layouts) == [0, 1] and len(layouts[1]) >= 2 and layouts[0] != layouts[1], layouts
-    assert any(off % 8 for off in offsets)   # views that start off a 16-byte boundary exist
+    buckets = master_weight.check_tables_match_ddp_buckets(
+        model, lambda pairs: segment_table([(g, p, opt.state[p]["master_param"], None)
+                                            for p, g in pairs]),
+        lambda p, g, chunk0: (g.data_ptr(), p.data_ptr(), opt.state[p]["master_param"].data_ptr(),
+                              0, g.numel(), chunk0), CHUNK)
+    # views that start off a 16-byte boundary exist
+    assert any(off % 8 for views in buckets for _, off, _ in views)
