@@ -185,6 +185,32 @@ def _check_max_grad_norm(max_grad_norm) -> Optional[float]:
     return float(max_grad_norm)
 
 
+def _check_sgd_args(lr, momentum, dampening, weight_decay, nesterov) -> None:
+    """torch.optim.SGD's checks and messages."""
+    if lr < 0.0:
+        raise ValueError(f"Invalid learning rate: {lr}")
+    if momentum < 0.0:
+        raise ValueError(f"Invalid momentum value: {momentum}")
+    if weight_decay < 0.0:
+        raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+    if nesterov and (momentum <= 0 or dampening != 0):
+        raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+
+
+def _check_adam_args(lr, betas, eps, weight_decay) -> None:
+    """torch.optim.Adam's checks and messages."""
+    if not 0.0 <= lr:
+        raise ValueError(f"Invalid learning rate: {lr}")
+    if not 0.0 <= eps:
+        raise ValueError(f"Invalid epsilon value: {eps}")
+    if not 0.0 <= betas[0] < 1.0:
+        raise ValueError(f"Invalid beta parameter at index 0: {betas[0]}")
+    if not 0.0 <= betas[1] < 1.0:
+        raise ValueError(f"Invalid beta parameter at index 1: {betas[1]}")
+    if not 0.0 <= weight_decay:
+        raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+
+
 class DynamicLossScale:
     """torch.amp.GradScaler's dynamic loss scale for the master-weight optimizers' `loss_scale=`.
 
@@ -279,6 +305,7 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
     into launches (_split) and launches one (_kernel)."""
 
     _FP32_STATE: Tuple[str, ...] = ("master_param",)   # state restored to fp32 by load_state_dict
+    _CPU_STEP = False                                    # load_state_dict gives `step` a CPU float32
     _FP32_HINT = ""                                      # the stock optimizer for fp32 parameters
     _CHUNK = CHUNK                                       # elements per chunk of the step's table
 
@@ -289,7 +316,7 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         self._tables: Dict[tuple, tuple] = {}        # launch key -> (rows, device table)
         self._stepped: set = set()                   # id(param) stepped (or normed) by a bucket
         self._streams: List[torch.cuda.Stream] = []  # streams those launches ran on
-        self._pending: List[tuple] = []              # clipping: (index, {group: pairs}) per bucket
+        self._pending: List[tuple] = []              # voted, not yet stepped: (where, {group: pairs})
         self._norms: Optional[torch.Tensor] = None   # clipping: fp32 norm per slot, on the device
         self._present: Optional[tuple] = None        # clipping: (slots, device index) of the last gather
         self.max_grad_norm = _check_max_grad_norm(max_grad_norm)
@@ -302,16 +329,23 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         self.table_uploads = 0
         super().__init__(params, defaults)
 
+    def _check_group(self, group: dict) -> None:
+        """A subclass's checks of one param group, defaults filled in, before its masters exist."""
+
     def add_param_group(self, param_group: dict) -> None:
         super().add_param_group(param_group)
         group = self.param_groups[-1]
-        for p in group["params"]:
-            if p.dtype not in _DTYPES or not _dense(p):
-                self.param_groups.pop()
-                raise ValueError("%s keeps fp32 masters of dense bf16 / f16 parameters; got a %s "
-                                 "parameter of shape %s and strides %s (fp32 parameters: %s)"
-                                 % (type(self).__name__, p.dtype, tuple(p.shape), p.stride(),
-                                    self._FP32_HINT))
+        try:
+            for p in group["params"]:
+                if p.dtype not in _DTYPES or not _dense(p):
+                    raise ValueError("%s keeps fp32 masters of dense bf16 / f16 parameters; got a %s "
+                                     "parameter of shape %s and strides %s (fp32 parameters: %s)"
+                                     % (type(self).__name__, p.dtype, tuple(p.shape), p.stride(),
+                                        self._FP32_HINT))
+            self._check_group(group)
+        except ValueError:
+            self.param_groups.pop()
+            raise
         for p in group["params"]:
             self._group_of[id(p)] = len(self.param_groups) - 1
             self._slot_of[id(p)] = len(self._slot_of)
@@ -319,7 +353,8 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                                                           memory_format=torch.preserve_format)
 
     def load_state_dict(self, state_dict: dict) -> None:
-        # Optimizer.load_state_dict casts floating state to the parameter's dtype: restore fp32
+        # Optimizer.load_state_dict casts floating state to the parameter's dtype: restore fp32, and a
+        # CPU float32 step of the optimizer's own, not the saved tensor, since step() counts in place
         super().load_state_dict(state_dict)
         params = [p for g in self.param_groups for p in g["params"]]
         for i, saved in state_dict["state"].items():
@@ -327,6 +362,9 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             for k in self._FP32_STATE:
                 if k in saved:
                     self.state[p][k] = saved[k].to(device=p.device, dtype=torch.float32, copy=True)
+            if self._CPU_STEP and "step" in saved:
+                self.state[p]["step"] = torch.as_tensor(saved["step"]).to("cpu", torch.float32,
+                                                                          copy=True)
 
     # ---- stepping ------------------------------------------------------------------------------
     def _split(self, group: dict, pairs) -> List[tuple]:
@@ -373,7 +411,6 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         """Step [(param, grad)] of one param group with the launches _split gives, on `stream` (which
         must then be current) or the current stream; with `coef`, clipped; with `inv_scale`,
         unscaled."""
-        self._check_pairs(pairs)
         stream = stream or torch.cuda.current_stream(pairs[0][0].device)
         for sub, entries, arg in self._split(group, pairs):
             if not entries:
@@ -409,27 +446,34 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             out.append((dtype, rows, chunks, self._table(key + (str(dtype),), rows, dev)))
         return out
 
-    def _launch_norms(self, pairs, key: tuple, norms: torch.Tensor,
-                      stream: torch.cuda.Stream) -> None:
-        """Enqueue on `stream` (current) the norms of [(param, grad)] into their slots of `norms`: one
-        tok_grad_norms call (two kernels) per gradient dtype.  With a loss scale, the norms of the
-        unscaled gradients (tok_grad_norms_unscaled), which also set this iteration's found_inf."""
-        scaled = self._scaling(norms.device) if self.loss_scale is not None else None
-        for dtype, rows, chunks, table in self._norm_tables(pairs, key, norms.device):
-            # caching-allocator scratch on `stream`: freed back to it after this call
-            partials = torch.empty(chunks, dtype=torch.float32, device=norms.device)
-            with torch.cuda.device(norms.device):
-                if scaled is None:
-                    _ffi.check(_ffi.lib().tok_grad_norms(
-                        C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype],
-                        C.c_void_p(partials.data_ptr() if chunks else 0),
-                        C.c_void_p(norms.data_ptr()), C.c_void_p(stream.cuda_stream)))
+    def _vote(self, pairs, where: tuple, dev: torch.device, stream: torch.cuda.Stream) -> None:
+        """Enqueue on `stream` (current) what step() must know of [(param, grad)] before any of them
+        steps, one call per gradient dtype: with max_grad_norm, their norms into their slots of the
+        norm buffer (tok_grad_norms, two kernels), or with a loss scale too the norms of the unscaled
+        gradients (tok_grad_norms_unscaled), which also set this iteration's found_inf; with a loss
+        scale alone, their inf / NaN check into found_inf (tok_grad_nonfinite)."""
+        clip = self.max_grad_norm is not None
+        norms = self._norm_buffer(dev) if clip else None
+        inv_scale, found_inf = self._scaling(dev) if self.loss_scale is not None else (None, None)
+        lib = _ffi.lib()
+        for dtype, rows, chunks, table in self._norm_tables(
+                pairs, ("norm" if clip else "check",) + where, dev):
+            args = (C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype])
+            with torch.cuda.device(dev):
+                if not clip:
+                    _ffi.check(lib.tok_grad_nonfinite(*args, C.c_void_p(found_inf.data_ptr()),
+                                                      C.c_void_p(stream.cuda_stream)))
+                    continue
+                # caching-allocator scratch on `stream`: freed back to it after this call
+                partials = torch.empty(chunks, dtype=torch.float32, device=dev)
+                partials_ptr = C.c_void_p(partials.data_ptr() if chunks else 0)
+                if inv_scale is None:
+                    _ffi.check(lib.tok_grad_norms(*args, partials_ptr, C.c_void_p(norms.data_ptr()),
+                                                  C.c_void_p(stream.cuda_stream)))
                 else:
-                    _ffi.check(_ffi.lib().tok_grad_norms_unscaled(
-                        C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype],
-                        C.c_void_p(scaled[0].data_ptr()),
-                        C.c_void_p(partials.data_ptr() if chunks else 0),
-                        C.c_void_p(norms.data_ptr()), C.c_void_p(scaled[1].data_ptr()),
+                    _ffi.check(lib.tok_grad_norms_unscaled(
+                        *args, C.c_void_p(inv_scale.data_ptr()), partials_ptr,
+                        C.c_void_p(norms.data_ptr()), C.c_void_p(found_inf.data_ptr()),
                         C.c_void_p(stream.cuda_stream)))
 
     # ---- loss scaling ----------------------------------------------------------------------------
@@ -440,57 +484,51 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
             self._found_inf = torch.zeros((), dtype=torch.float32, device=dev)
         return self.loss_scale.inv_scale, self._found_inf
 
-    def _launch_check(self, pairs, key: tuple, dev: torch.device,
-                      stream: torch.cuda.Stream) -> None:
-        """Enqueue on `stream` (current) the inf / NaN check of [(param, grad)] into this iteration's
-        found_inf: one tok_grad_nonfinite launch per gradient dtype."""
-        _, found_inf = self._scaling(dev)
-        for dtype, rows, chunks, table in self._norm_tables(pairs, key, dev):
-            with torch.cuda.device(dev):
-                _ffi.check(_ffi.lib().tok_grad_nonfinite(
-                    C.c_void_p(table.data_ptr()), len(rows), chunks, _DTYPES[dtype],
-                    C.c_void_p(found_inf.data_ptr()), C.c_void_p(stream.cuda_stream)))
-
     def _next_iteration(self, found_inf: torch.Tensor) -> None:
         """GradScaler.update with this iteration's verdict, then a zeroed found_inf for the next."""
         self.loss_scale._update(found_inf)
         self.found_inf = found_inf
         self._found_inf = torch.zeros((), dtype=torch.float32, device=found_inf.device)
 
-    def _deferred_step(self) -> None:
-        """step() with max_grad_norm or a loss scale, on the current stream after the bucket streams:
-        the norms or inf / NaN checks no bucket covered; with clipping, clip_grad_norm_'s total and
-        coefficient; with a loss scale, GradScaler's host read of found_inf; then every clipped or
-        unscaled launch unless an inf or NaN was found; then the scale's update."""
-        pending, self._pending = self._pending, []
-        rest = []
-        for gi, group in enumerate(self.param_groups):
-            pairs = [(p, p.grad) for p in group["params"]
-                     if p.grad is not None and id(p) not in self._stepped]
-            if pairs:
-                rest.append((gi, pairs))
-        present = tuple(self._slot_of[id(p)] for group in self.param_groups for p in group["params"]
-                        if id(p) in self._stepped or p.grad is not None)
-        self._stepped.clear()
-        self._streams.clear()
+    # ---- stepping paths --------------------------------------------------------------------------
+    def _enqueue(self, by_group: Dict[int, list], where: tuple,
+                 stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Take [(param, grad)] per param group index, of gradient bucket `index` (`where` is
+        ("bucket", index)) or of what no bucket covered (("group",)), on `stream` or the current
+        stream.  Without max_grad_norm or a loss scale, step them; otherwise enqueue their vote and
+        keep them for _finish."""
+        pairs = [pg for prs in by_group.values() for pg in prs]
+        self._check_pairs(pairs)
+        with torch.cuda.stream(stream):
+            if self.max_grad_norm is None and self.loss_scale is None:
+                for gi, prs in by_group.items():
+                    self._launch(self.param_groups[gi], prs, where + (gi,), stream)
+            else:
+                dev = pairs[0][0].device
+                self._vote(pairs, where, dev, stream or torch.cuda.current_stream(dev))
+                self._pending.append((where, by_group))
+        self._stepped.update(id(p) for p, _ in pairs)
+
+    def _finish(self) -> None:
+        """step() with max_grad_norm or a loss scale, on the current stream after every vote: with
+        clipping, clip_grad_norm_'s total and coefficient; with a loss scale, GradScaler's host read
+        of found_inf; then every pending clipped or unscaled launch, in arrival order, unless an inf
+        or NaN was found; then the scale's update."""
         clip, scaling = self.max_grad_norm is not None, self.loss_scale is not None
         self.step_skipped = False
-        if not present:
+        if not self._pending:
             if clip:
                 self.grad_norm = torch.tensor(0.0)   # what clip_grad_norm_ returns without gradients
             # the scale stays: GradScaler.update refuses to run without any inf check recorded
             return
-        pairs = [pg for _, prs in rest for pg in prs]
-        self._check_pairs(pairs)
-        dev = (pairs[0][0] if pairs else next(iter(pending[0][1].values()))[0][0]).device
-        stream = torch.cuda.current_stream(dev)
+        dev = next(iter(self._pending[0][1].values()))[0][0].device
         inv_scale = found_inf = coef = None
         if scaling:
             inv_scale, found_inf = self._scaling(dev)
         if clip:
             norms = self._norm_buffer(dev)
-            if pairs:
-                self._launch_norms(pairs, ("norm", "group"), norms, stream)
+            present = tuple(self._slot_of[id(p)] for group in self.param_groups
+                            for p in group["params"] if id(p) in self._stepped)
             if len(present) != norms.numel():
                 # clip_grad_norm_ stacks only the gradients that exist: gather their slots, in order
                 if self._present is None or self._present[0] != present:
@@ -509,18 +547,13 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                     "set `error_if_nonfinite=False`")
             coef = torch.clamp(self.max_grad_norm / (total + 1e-6), max=1.0)
             self.grad_norm = total
-        elif pairs:
-            self._launch_check(pairs, ("check", "group"), dev, stream)
         if scaling and found_inf.item():   # GradScaler._maybe_opt_step's host read
             self.step_skipped = True
         else:
-            for index, by_group in pending:
+            for where, by_group in self._pending:
                 for gi, prs in by_group.items():
-                    self._launch(self.param_groups[gi], prs, ("clip bucket", index, gi), stream,
-                                 coef, inv_scale)
-            for gi, prs in rest:
-                self._launch(self.param_groups[gi], prs, ("clip group", gi), stream, coef,
-                             inv_scale)
+                    self._launch(self.param_groups[gi], prs, ("clip",) + where + (gi,), coef=coef,
+                                 inv_scale=inv_scale)
         if scaling:
             self._next_iteration(found_inf)
 
@@ -542,26 +575,8 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                 by_group.setdefault(gi, []).append((p, g))
         if not by_group:
             return
-        dev = next(iter(by_group.values()))[0][0].device
-        stream = stream or torch.cuda.current_stream(dev)
-        if self.max_grad_norm is not None or self.loss_scale is not None:
-            pairs = [pg for prs in by_group.values() for pg in prs]
-            self._check_pairs(pairs)
-            with torch.cuda.stream(stream):
-                if self.max_grad_norm is not None:
-                    self._launch_norms(pairs, ("norm", "bucket", index), self._norm_buffer(dev),
-                                       stream)
-                else:
-                    self._launch_check(pairs, ("check", "bucket", index), dev, stream)
-            self._pending.append((index, by_group))
-            self._stepped.update(id(p) for p, _ in pairs)
-            if stream not in self._streams:
-                self._streams.append(stream)
-            return
-        with torch.cuda.stream(stream):
-            for gi, pairs in by_group.items():
-                self._launch(self.param_groups[gi], pairs, ("bucket", index, gi), stream)
-                self._stepped.update(id(p) for p, _ in pairs)
+        stream = stream or torch.cuda.current_stream(next(iter(by_group.values()))[0][0].device)
+        self._enqueue(by_group, ("bucket", index), stream)
         if stream not in self._streams:
             self._streams.append(stream)
 
@@ -573,27 +588,22 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                 loss = closure()
         for s in self._streams:
             torch.cuda.current_stream(s.device).wait_stream(s)
-        if self.max_grad_norm is not None or self.loss_scale is not None:
-            self._deferred_step()
-            return loss
-        for gi, group in enumerate(self.param_groups):
-            pairs = [(p, p.grad) for p in group["params"]
-                     if p.grad is not None and id(p) not in self._stepped]
-            if pairs:
-                self._launch(group, pairs, ("group", gi))
-        self._stepped.clear()
-        self._streams.clear()
+        try:
+            rest = {}
+            for gi, group in enumerate(self.param_groups):
+                pairs = [(p, p.grad) for p in group["params"]
+                         if p.grad is not None and id(p) not in self._stepped]
+                if pairs:
+                    rest[gi] = pairs
+            if rest:
+                self._enqueue(rest, ("group",))
+            if self.max_grad_norm is not None or self.loss_scale is not None:
+                self._finish()
+        finally:
+            self._stepped.clear()
+            self._streams.clear()
+            self._pending.clear()
         return loss
-
-
-def _own_cpu_steps(opt: _MasterWeightOptimizer, state_dict: dict) -> None:
-    """After load_state_dict: a CPU float32 step of the optimizer's own, not the saved tensor, since
-    step() counts in place."""
-    params = [p for g in opt.param_groups for p in g["params"]]
-    for i, saved in state_dict["state"].items():
-        if "step" in saved:
-            opt.state[params[i]]["step"] = torch.as_tensor(saved["step"]).to(
-                "cpu", torch.float32, copy=True)
 
 
 def _split_by_step(opt: _MasterWeightOptimizer, pairs, amsgrad: bool) -> List[tuple]:
@@ -618,6 +628,31 @@ def _split_by_step(opt: _MasterWeightOptimizer, pairs, amsgrad: bool) -> List[tu
     return [(i, entries, step) for i, ((step, _), entries) in enumerate(ordered)]
 
 
+def _master_step(name: str, args: list, stream: torch.cuda.Stream, coef: Optional[torch.Tensor],
+                 inv_scale: Optional[torch.Tensor]) -> None:
+    """One launch of tok_sgd_master_step or tok_adam_master_step (`name`) with its common `args`:
+    with `inv_scale` the _unscaled entry point, clipped too with `coef`; otherwise with `coef` the
+    _clipped one; otherwise the plain one."""
+    lib = _ffi.lib()
+    if inv_scale is not None:
+        _ffi.check(getattr(lib, name + "_unscaled")(
+            *args, C.c_void_p(inv_scale.data_ptr()),
+            C.c_void_p(0 if coef is None else coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
+    elif coef is None:
+        _ffi.check(getattr(lib, name)(*args, C.c_void_p(stream.cuda_stream)))
+    else:
+        _ffi.check(getattr(lib, name + "_clipped")(
+            *args, C.c_void_p(coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
+
+
+def _sgd_kernel(group, table, count, chunks, dtype, fresh, stream, coef, inv_scale) -> None:
+    """MasterWeightSGD's _kernel, also MasterWeightLARS's for its lars=False groups."""
+    _master_step("tok_sgd_master_step",
+                 [C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], group["momentum"],
+                  group["dampening"], group["weight_decay"], int(group["nesterov"]), fresh],
+                 stream, coef, inv_scale)
+
+
 class MasterWeightSGD(_MasterWeightOptimizer):
     _FP32_STATE = ("master_param", "momentum_buffer")
     _FP32_HINT = "torch.optim.SGD(fused=True)"
@@ -626,14 +661,7 @@ class MasterWeightSGD(_MasterWeightOptimizer):
                  weight_decay: float = 0.0, nesterov: bool = False, *, maximize: bool = False,
                  differentiable: bool = False, max_grad_norm: Optional[float] = None,
                  error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
-        if lr < 0.0:
-            raise ValueError("Invalid learning rate: %r" % lr)
-        if momentum < 0.0:
-            raise ValueError("Invalid momentum value: %r" % momentum)
-        if weight_decay < 0.0:
-            raise ValueError("Invalid weight_decay value: %r" % weight_decay)
-        if nesterov and (momentum <= 0 or dampening != 0):
-            raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+        _check_sgd_args(lr, momentum, dampening, weight_decay, nesterov)
         if maximize or differentiable:
             raise ValueError("MasterWeightSGD supports neither maximize nor differentiable")
         super().__init__(params, dict(lr=lr, momentum=momentum, dampening=dampening,
@@ -655,24 +683,14 @@ class MasterWeightSGD(_MasterWeightOptimizer):
             old.append((g, p, st["master_param"], m))
         return [(1, fresh, 1), (0, old, 0)]
 
-    def _kernel(self, group, table, count, chunks, dtype, fresh, stream, coef, inv_scale) -> None:
-        args = [C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], group["momentum"],
-                group["dampening"], group["weight_decay"], int(group["nesterov"]), fresh]
-        if inv_scale is not None:
-            _ffi.check(_ffi.lib().tok_sgd_master_step_unscaled(
-                *args, C.c_void_p(inv_scale.data_ptr()),
-                C.c_void_p(0 if coef is None else coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
-        elif coef is None:
-            _ffi.check(_ffi.lib().tok_sgd_master_step(*args, C.c_void_p(stream.cuda_stream)))
-        else:
-            _ffi.check(_ffi.lib().tok_sgd_master_step_clipped(
-                *args, C.c_void_p(coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
+    _kernel = staticmethod(_sgd_kernel)
 
 
 class MasterWeightAdam(_MasterWeightOptimizer):
     """torch.optim.Adam (foreach) on fp32 masters; `decoupled_weight_decay=True` is AdamW."""
 
     _FP32_STATE = ("master_param", "exp_avg", "exp_avg_sq", "max_exp_avg_sq")
+    _CPU_STEP = True
     _FP32_HINT = "torch.optim.Adam(fused=True)"
 
     def __init__(self, params, lr: float = 1e-3, betas: Tuple[float, float] = (0.9, 0.999),
@@ -687,43 +705,22 @@ class MasterWeightAdam(_MasterWeightOptimizer):
         if maximize or capturable or differentiable or fused:
             raise ValueError("%s supports none of maximize, capturable, differentiable and fused"
                              % name)
-        # torch.optim.Adam's checks and messages
-        if not 0.0 <= lr:
-            raise ValueError(f"Invalid learning rate: {lr}")
-        if not 0.0 <= eps:
-            raise ValueError(f"Invalid epsilon value: {eps}")
-        if not 0.0 <= betas[0] < 1.0:
-            raise ValueError(f"Invalid beta parameter at index 0: {betas[0]}")
-        if not 0.0 <= betas[1] < 1.0:
-            raise ValueError(f"Invalid beta parameter at index 1: {betas[1]}")
-        if not 0.0 <= weight_decay:
-            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        _check_adam_args(lr, betas, eps, weight_decay)
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay,
                                       amsgrad=amsgrad,
                                       decoupled_weight_decay=decoupled_weight_decay),
                          max_grad_norm, error_if_nonfinite, loss_scale)
-
-    def load_state_dict(self, state_dict: dict) -> None:
-        super().load_state_dict(state_dict)
-        _own_cpu_steps(self, state_dict)
 
     def _split(self, group: dict, pairs) -> List[tuple]:
         return _split_by_step(self, pairs, group["amsgrad"])
 
     def _kernel(self, group, table, count, chunks, dtype, step, stream, coef, inv_scale) -> None:
         beta1, beta2 = group["betas"]
-        args = [C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], beta1, beta2,
-                group["eps"], group["weight_decay"], int(group["decoupled_weight_decay"]),
-                int(group["amsgrad"]), step]
-        if inv_scale is not None:
-            _ffi.check(_ffi.lib().tok_adam_master_step_unscaled(
-                *args, C.c_void_p(inv_scale.data_ptr()),
-                C.c_void_p(0 if coef is None else coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
-        elif coef is None:
-            _ffi.check(_ffi.lib().tok_adam_master_step(*args, C.c_void_p(stream.cuda_stream)))
-        else:
-            _ffi.check(_ffi.lib().tok_adam_master_step_clipped(
-                *args, C.c_void_p(coef.data_ptr()), C.c_void_p(stream.cuda_stream)))
+        _master_step("tok_adam_master_step",
+                     [C.c_void_p(table.data_ptr()), count, chunks, dtype, group["lr"], beta1, beta2,
+                      group["eps"], group["weight_decay"], int(group["decoupled_weight_decay"]),
+                      int(group["amsgrad"]), step],
+                     stream, coef, inv_scale)
 
 
 class MasterWeightAdamW(MasterWeightAdam):
@@ -750,6 +747,7 @@ class MasterWeightLAMB(_MasterWeightOptimizer):
     parameter's master and update, not a global norm."""
 
     _FP32_STATE = ("master_param", "exp_avg", "exp_avg_sq")
+    _CPU_STEP = True
     _FP32_HINT = "torch.optim has no LAMB to use instead"
     _CHUNK = NORM_CHUNK   # _foreach_norm's chunks: the trust ratio's norms keep its reduction
 
@@ -764,23 +762,9 @@ class MasterWeightLAMB(_MasterWeightOptimizer):
         if amsgrad or maximize or capturable or differentiable or fused:
             raise ValueError("%s supports none of amsgrad, maximize, capturable, differentiable and "
                              "fused" % name)
-        # torch.optim.Adam's checks and messages
-        if not 0.0 <= lr:
-            raise ValueError(f"Invalid learning rate: {lr}")
-        if not 0.0 <= eps:
-            raise ValueError(f"Invalid epsilon value: {eps}")
-        if not 0.0 <= betas[0] < 1.0:
-            raise ValueError(f"Invalid beta parameter at index 0: {betas[0]}")
-        if not 0.0 <= betas[1] < 1.0:
-            raise ValueError(f"Invalid beta parameter at index 1: {betas[1]}")
-        if not 0.0 <= weight_decay:
-            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        _check_adam_args(lr, betas, eps, weight_decay)
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay),
                          max_grad_norm, error_if_nonfinite, loss_scale)
-
-    def load_state_dict(self, state_dict: dict) -> None:
-        super().load_state_dict(state_dict)
-        _own_cpu_steps(self, state_dict)
 
     def _split(self, group: dict, pairs) -> List[tuple]:
         """Adam's: one launch per (step count, dtype), entries without max_exp_avg_sq."""
@@ -811,14 +795,8 @@ def _check_lars_group(group: dict) -> None:
     for k in ("lr", "momentum", "dampening", "weight_decay", "trust_coefficient", "eps"):
         if isinstance(group[k], (bool, torch.Tensor)) or not isinstance(group[k], (int, float)):
             raise ValueError("MasterWeightLARS takes %s as a Python float, got %r" % (k, group[k]))
-    if group["lr"] < 0.0:
-        raise ValueError(f"Invalid learning rate: {group['lr']}")
-    if group["momentum"] < 0.0:
-        raise ValueError(f"Invalid momentum value: {group['momentum']}")
-    if group["weight_decay"] < 0.0:
-        raise ValueError(f"Invalid weight_decay value: {group['weight_decay']}")
-    if group["nesterov"] and (group["momentum"] <= 0 or group["dampening"] != 0):
-        raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+    _check_sgd_args(group["lr"], group["momentum"], group["dampening"], group["weight_decay"],
+                    group["nesterov"])
     for k in ("lr", "momentum", "dampening", "weight_decay", "trust_coefficient", "eps"):
         if not (math.isfinite(group[k]) and group[k] >= 0.0):
             raise ValueError(f"Invalid {k} value: {group[k]}")
@@ -849,17 +827,7 @@ class MasterWeightLARS(_MasterWeightOptimizer):
         _check_lars_group(defaults)
         super().__init__(params, defaults, max_grad_norm, error_if_nonfinite, loss_scale)
 
-    def add_param_group(self, param_group: dict) -> None:
-        super().add_param_group(param_group)
-        try:
-            _check_lars_group(self.param_groups[-1])
-        except ValueError:
-            group = self.param_groups.pop()
-            for p in group["params"]:
-                self._group_of.pop(id(p), None)
-                self._slot_of.pop(id(p), None)
-                self.state.pop(p, None)
-            raise
+    _check_group = staticmethod(_check_lars_group)
 
     def _chunk(self, group: dict) -> int:
         # _foreach_norm's chunks where the trust ratio's norms keep its reduction
@@ -869,8 +837,7 @@ class MasterWeightLARS(_MasterWeightOptimizer):
 
     def _kernel(self, group, table, count, chunks, dtype, fresh, stream, coef, inv_scale) -> None:
         if not group["lars"]:
-            MasterWeightSGD._kernel(self, group, table, count, chunks, dtype, fresh, stream, coef,
-                                    inv_scale)
+            _sgd_kernel(group, table, count, chunks, dtype, fresh, stream, coef, inv_scale)
             return
         # caching-allocator scratch on `stream` (current): the two norm partials of every chunk
         partials = torch.empty(2 * chunks, dtype=torch.float32, device=table.device)
