@@ -230,7 +230,11 @@ int tok_bn_stats_fwd(const void* x, int64_t rows, int channels, double momentum,
  * Activations and the workspace must be 16-byte aligned and channels a multiple of 8
  * (TOK_ERR_ALIGN); rows * channels must stay below 2^31 (TOK_ERR_INVALID).  Enqueued on
  * `cuda_stream` (three launches at most), no synchronisation; TOK_ERR_NO_DEVICE without a GPU.
- * tok_bn_bwd_workspace_bytes returns the byte count, or a TOK_ERR_* code for a refused shape. */
+ * tok_bn_bwd_workspace_bytes returns the byte count, or a TOK_ERR_* code for a refused shape.
+ * tok_bn_add_relu_bwd2 and tok_bn2_add_relu_bwd2 take y's gradient in two halves, gy and gy2 (a
+ * residual block's output feeds two consumers), and are bit-identical to the calls above with
+ * gy = gy + gy2 as ATen adds two bf16 tensors; the sum is formed in the reduction and not stored.
+ * gy2 is checked as gy is (not NULL, 16-byte aligned); the workspace is the same. */
 int64_t tok_bn_bwd_workspace_bytes(int64_t rows, int channels, int mode);
 int tok_bn_relu_bwd(const void* gy, const void* x, const float* mean, const float* invstd,
                     const void* weight, const void* bias, void* dx, void* grad_weight,
@@ -245,6 +249,16 @@ int tok_bn2_add_relu_bwd(const void* gy, const void* y, const void* x, const flo
                          void* dx, void* grad_weight, void* grad_bias, void* dxd,
                          void* grad_weight_d, void* grad_bias_d, int64_t rows, int channels,
                          void* workspace, void* cuda_stream);
+int tok_bn_add_relu_bwd2(const void* gy, const void* gy2, const void* y, const void* x,
+                         const float* mean, const float* invstd, const void* weight, void* dz,
+                         void* dx, void* grad_weight, void* grad_bias, int64_t rows, int channels,
+                         void* workspace, void* cuda_stream);
+int tok_bn2_add_relu_bwd2(const void* gy, const void* gy2, const void* y, const void* x,
+                          const float* mean, const float* invstd, const void* weight,
+                          const void* xd, const float* mean_d, const float* invstd_d,
+                          const void* weight_d, void* dz, void* dx, void* grad_weight,
+                          void* grad_bias, void* dxd, void* grad_weight_d, void* grad_bias_d,
+                          int64_t rows, int channels, void* workspace, void* cuda_stream);
 
 /* Max pool with kernel 3, stride 2, padding 1 (ResNet's stem; torch_on_k8s_b200/fused_bn.py's
  * max_pool) of an NHWC bf16 activation [n, h, w, channels], bit-identical to ATen's channels_last

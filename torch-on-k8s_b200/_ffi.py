@@ -118,6 +118,8 @@ PROTOTYPES = {
     "tok_bn_relu_bwd": (C.c_int, [_P] * 9 + [C.c_int64, C.c_int, _P, _P]),
     "tok_bn_add_relu_bwd": (C.c_int, [_P] * 10 + [C.c_int64, C.c_int, _P, _P]),
     "tok_bn2_add_relu_bwd": (C.c_int, [_P] * 17 + [C.c_int64, C.c_int, _P, _P]),
+    "tok_bn_add_relu_bwd2": (C.c_int, [_P] * 11 + [C.c_int64, C.c_int, _P, _P]),
+    "tok_bn2_add_relu_bwd2": (C.c_int, [_P] * 18 + [C.c_int64, C.c_int, _P, _P]),
     "tok_max_pool_fwd": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, C.c_int64, C.c_int, _P]),
     "tok_max_pool_bwd": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, C.c_int64, C.c_int, _P]),
     "tok_sgd_master_step": (C.c_int, [_P, C.c_int, C.c_int64, C.c_int, C.c_double, C.c_double,

@@ -370,6 +370,13 @@ __global__ void __launch_bounds__(kStatsThreads) bn_stats_finish_kernel(const St
 // ---- backward ---------------------------------------------------------------------------------
 // threshold_backward(gy, y, 0) and native_batch_norm_backward in one reduction and one elementwise
 // pass.  The mask is threshold_backward's: dz = (v <= 0) ? +0 : gy, so a NaN v passes gy and ±0 masks.
+// Modes 1 and 2 may take y's gradient in two halves (a residual block's output feeds both the next
+// block's conv1 and its shortcut): the reduction then forms gy = bf16(f(gy) + f(gy2)) per element
+// before the mask, which is what autograd's sum of the two, ATen's CUDAFunctor_add<BFloat16> with
+// alpha 1, computes.  Its sm_90 code is one float add of the widened operands (a fma by alpha = 1
+// rounds the same way) and one round-to-nearest-even conversion: NaN in either operand gives the
+// canonical NaN, inf + -inf the canonical NaN, -0 + -0 = -0, +0 + -0 = +0, and a sum past bf16's
+// range rounds to inf.  Every case is symmetric, so which half autograd holds first does not matter.
 // The arithmetic is that of ATen's batch_norm_backward_reduce_channels_last_kernel<4, BFloat16, float,
 // BFloat16> and batch_norm_backward_elemt_channels_last_kernel, pinned as the sm_90 code of torch's
 // libtorch_cuda.so performs it (cuobjdump -sass):
@@ -402,6 +409,7 @@ struct BwdArgs {
   BwdSide a;                       // the main batch norm
   BwdSide d;                       // mode 2: the downsample batch norm
   const uint4* gy;
+  const uint4* gy2;                // modes 1, 2: y's second gradient, summed with gy (may be null)
   const uint4* y;                  // modes 1, 2: the saved output, the mask's v
   uint4* dz;                       // modes 1, 2: the masked gradient, written by the reduction
   const __nv_bfloat16* bias;       // mode 0: for the recomputed v
@@ -417,9 +425,10 @@ struct BwdArgs {
 };
 
 constexpr int kBwdPartialThreads = 512;  // physical threads per block of the reduction
-// chain steps loaded ahead of the one computed (mode 2 loads four streams a step)
+// chain steps loaded ahead of the one computed (mode 2 loads four streams a step, five with gy2)
 template <int kMode>
 constexpr int kBwdDepth = kMode == 2 ? 2 : 4;
+constexpr int kBwdStreams = 5;           // gy, x, y, xd, gy2
 
 __device__ __forceinline__ float relu_grad(float g, float v) { return v <= 0.0f ? 0.0f : g; }
 
@@ -435,17 +444,20 @@ __device__ __forceinline__ void load_bwd_column(const BwdSide& s, const __nv_bfl
   }
 }
 
-// q = {gy, x, y, xd} of row r, zeros past the last row
-template <int kMode>
-__device__ __forceinline__ void load_bwd_row(const BwdArgs& a, int v, int64_t r, uint4 (&q)[4]) {
+// q = {gy, x, y, xd, gy2} of row r, zeros past the last row
+template <int kMode, bool kTwo>
+__device__ __forceinline__ void load_bwd_row(const BwdArgs& a, int v, int64_t r,
+                                             uint4 (&q)[kBwdStreams]) {
   const uint4 zero = make_uint4(0, 0, 0, 0);
-  q[0] = q[1] = q[2] = q[3] = zero;
+#pragma unroll
+  for (int t = 0; t < kBwdStreams; ++t) q[t] = zero;
   if (r < a.rows) {
     const int64_t i = r * a.vecs + v;
     q[0] = __ldg(a.gy + i);
     q[1] = __ldg(a.a.x + i);
     if (kMode != 0) q[2] = __ldg(a.y + i);
     if (kMode == 2) q[3] = __ldg(a.d.x + i);
+    if (kTwo) q[4] = __ldg(a.gy2 + i);
   }
 }
 
@@ -464,8 +476,9 @@ __device__ __forceinline__ void bwd_finish(const BwdArgs& a, int c, float dy, fl
 }
 
 // blockDim = (4 * tile, block_y): lane j = threadIdx.x % 4 of thread (vx = threadIdx.x / 4, ty) of
-// block (bx, by) runs chain j of logical thread (by, ty) on vector bx * tile + vx.
-template <int kMode>
+// block (bx, by) runs chain j of logical thread (by, ty) on vector bx * tile + vx.  kTwo: gy is the
+// sum of gy and gy2.
+template <int kMode, bool kTwo>
 __global__ void __launch_bounds__(kBwdPartialThreads) bn_bwd_partial_kernel(const BwdArgs a) {
   constexpr int kSlots = kBwdPartialThreads / kStatsChains;
   __shared__ float s_dy[kSlots][kVec];
@@ -487,25 +500,27 @@ __global__ void __launch_bounds__(kBwdPartialThreads) bn_bwd_partial_kernel(cons
     Column ca, cd;
     load_bwd_column(a.a, kMode == 0 ? a.bias : nullptr, v, ca);
     if (kMode == 2) load_bwd_column(a.d, nullptr, v, cd);
-    uint4 buf[kBwdDepth<kMode>][4];
+    uint4 buf[kBwdDepth<kMode>][kBwdStreams];
 #pragma unroll
-    for (int s = 0; s < kBwdDepth<kMode>; ++s) load_bwd_row<kMode>(a, v, p + s * step, buf[s]);
+    for (int s = 0; s < kBwdDepth<kMode>; ++s) load_bwd_row<kMode, kTwo>(a, v, p + s * step, buf[s]);
     for (int i0 = 0; i0 < a.loop_count; i0 += kBwdDepth<kMode>) {
 #pragma unroll
       for (int s = 0; s < kBwdDepth<kMode>; ++s) {
         if (i0 + s < a.loop_count) {
           const int64_t row = p + (int64_t)(i0 + s) * step;
-          uint4 q[4];
+          uint4 q[kBwdStreams];
 #pragma unroll
-          for (int t = 0; t < 4; ++t) q[t] = buf[s][t];
-          load_bwd_row<kMode>(a, v, row + kBwdDepth<kMode> * step, buf[s]);
+          for (int t = 0; t < kBwdStreams; ++t) q[t] = buf[s][t];
+          load_bwd_row<kMode, kTwo>(a, v, row + kBwdDepth<kMode> * step, buf[s]);
           uint32_t dz_bits[4];
 #pragma unroll
           for (int k = 0; k < kVec; ++k) {
             const int w = k >> 1, h = k & 1;
             const float x = widen(word(q[1], w), h);
             const float v_mask = kMode == 0 ? bn_apply(x, ca, k) : widen(word(q[2], w), h);
-            const float dz = relu_grad(widen(word(q[0], w), h), v_mask);
+            float g = widen(word(q[0], w), h);
+            if (kTwo) g = __uint_as_float(bf16_bits(__fadd_rn(g, widen(word(q[4], w), h))) << 16);
+            const float dz = relu_grad(g, v_mask);
             dy[k] = __fadd_rn(dy[k], dz);
             xmu[k] = __fmaf_rn(__fsub_rn(x, ca.mean[k]), dz, xmu[k]);
             if (kMode == 2)
@@ -812,12 +827,13 @@ BwdSide bwd_side(const void* x, const float* mean, const float* invstd, const vo
 }
 
 // Checks what every mode shares, lays the workspace out and runs the reduction, its finish and
-// (when a dx is asked for) the elementwise pass.
-template <int kMode>
+// (when a dx is asked for) the elementwise pass.  kTwo: y's gradient comes in two halves, gy + gy2.
+template <int kMode, bool kTwo>
 int bn_bwd(const char* who, BwdArgs& a, int64_t rows, int channels, void* workspace,
            void* cuda_stream) {
   int rc = check_stats_shape(who, rows, channels);
   if (rc == TOK_OK) rc = check_act(who, "gy", a.gy, true);
+  if (rc == TOK_OK && kTwo) rc = check_act(who, "gy2", a.gy2, true);
   if (rc == TOK_OK) rc = check_act(who, "x", a.a.x, true);
   if (rc == TOK_OK) rc = check_act(who, "dx", a.a.dx, false);
   if (rc == TOK_OK && kMode != 0) rc = check_act(who, "y", a.y, true);
@@ -855,8 +871,8 @@ int bn_bwd(const char* who, BwdArgs& a, int64_t rows, int channels, void* worksp
   int tile = kBwdPartialThreads / (kStatsChains * g.block_y);
   if (tile > a.vecs) tile = a.vecs;
   cudaStream_t st = (cudaStream_t)cuda_stream;
-  bn_bwd_partial_kernel<kMode><<<dim3((a.vecs + tile - 1) / tile, g.grid_y),
-                                 dim3(kStatsChains * tile, g.block_y), 0, st>>>(a);
+  bn_bwd_partial_kernel<kMode, kTwo><<<dim3((a.vecs + tile - 1) / tile, g.grid_y),
+                                       dim3(kStatsChains * tile, g.block_y), 0, st>>>(a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(TOK_ERR_CUDA, "bn_bwd_partial launch: %s", cudaGetErrorString(e));
   if (g.grid_y > 1) {
@@ -1008,19 +1024,59 @@ extern "C" int tok_bn_relu_bwd(const void* gy, const void* x, const float* mean,
   a.a = bwd_side(x, mean, invstd, weight, dx, grad_weight, grad_bias);
   a.gy = (const uint4*)gy;
   a.bias = (const __nv_bfloat16*)bias;
-  return bn_bwd<0>("tok_bn_relu_bwd", a, rows, channels, workspace, cuda_stream);
+  return bn_bwd<0, false>("tok_bn_relu_bwd", a, rows, channels, workspace, cuda_stream);
 }
+
+namespace {
+
+template <bool kTwo>
+int bn_add_relu_bwd(const char* who, const void* gy, const void* gy2, const void* y, const void* x,
+                    const float* mean, const float* invstd, const void* weight, void* dz, void* dx,
+                    void* grad_weight, void* grad_bias, int64_t rows, int channels,
+                    void* workspace, void* cuda_stream) {
+  BwdArgs a{};
+  a.a = bwd_side(x, mean, invstd, weight, dx, grad_weight, grad_bias);
+  a.gy = (const uint4*)gy;
+  a.gy2 = (const uint4*)gy2;
+  a.y = (const uint4*)y;
+  a.dz = (uint4*)dz;
+  return bn_bwd<1, kTwo>(who, a, rows, channels, workspace, cuda_stream);
+}
+
+template <bool kTwo>
+int bn2_add_relu_bwd(const char* who, const void* gy, const void* gy2, const void* y,
+                     const void* x, const float* mean, const float* invstd, const void* weight,
+                     const void* xd, const float* mean_d, const float* invstd_d,
+                     const void* weight_d, void* dz, void* dx, void* grad_weight, void* grad_bias,
+                     void* dxd, void* grad_weight_d, void* grad_bias_d, int64_t rows, int channels,
+                     void* workspace, void* cuda_stream) {
+  BwdArgs a{};
+  a.a = bwd_side(x, mean, invstd, weight, dx, grad_weight, grad_bias);
+  a.d = bwd_side(xd, mean_d, invstd_d, weight_d, dxd, grad_weight_d, grad_bias_d);
+  a.gy = (const uint4*)gy;
+  a.gy2 = (const uint4*)gy2;
+  a.y = (const uint4*)y;
+  a.dz = (uint4*)dz;
+  return bn_bwd<2, kTwo>(who, a, rows, channels, workspace, cuda_stream);
+}
+
+}  // namespace
 
 extern "C" int tok_bn_add_relu_bwd(const void* gy, const void* y, const void* x, const float* mean,
                                    const float* invstd, const void* weight, void* dz, void* dx,
                                    void* grad_weight, void* grad_bias, int64_t rows, int channels,
                                    void* workspace, void* cuda_stream) {
-  BwdArgs a{};
-  a.a = bwd_side(x, mean, invstd, weight, dx, grad_weight, grad_bias);
-  a.gy = (const uint4*)gy;
-  a.y = (const uint4*)y;
-  a.dz = (uint4*)dz;
-  return bn_bwd<1>("tok_bn_add_relu_bwd", a, rows, channels, workspace, cuda_stream);
+  return bn_add_relu_bwd<false>("tok_bn_add_relu_bwd", gy, nullptr, y, x, mean, invstd, weight, dz,
+                                dx, grad_weight, grad_bias, rows, channels, workspace, cuda_stream);
+}
+
+extern "C" int tok_bn_add_relu_bwd2(const void* gy, const void* gy2, const void* y, const void* x,
+                                    const float* mean, const float* invstd, const void* weight,
+                                    void* dz, void* dx, void* grad_weight, void* grad_bias,
+                                    int64_t rows, int channels, void* workspace,
+                                    void* cuda_stream) {
+  return bn_add_relu_bwd<true>("tok_bn_add_relu_bwd2", gy, gy2, y, x, mean, invstd, weight, dz, dx,
+                               grad_weight, grad_bias, rows, channels, workspace, cuda_stream);
 }
 
 extern "C" int tok_bn2_add_relu_bwd(const void* gy, const void* y, const void* x, const float* mean,
@@ -1030,11 +1086,20 @@ extern "C" int tok_bn2_add_relu_bwd(const void* gy, const void* y, const void* x
                                     void* grad_bias, void* dxd, void* grad_weight_d,
                                     void* grad_bias_d, int64_t rows, int channels, void* workspace,
                                     void* cuda_stream) {
-  BwdArgs a{};
-  a.a = bwd_side(x, mean, invstd, weight, dx, grad_weight, grad_bias);
-  a.d = bwd_side(xd, mean_d, invstd_d, weight_d, dxd, grad_weight_d, grad_bias_d);
-  a.gy = (const uint4*)gy;
-  a.y = (const uint4*)y;
-  a.dz = (uint4*)dz;
-  return bn_bwd<2>("tok_bn2_add_relu_bwd", a, rows, channels, workspace, cuda_stream);
+  return bn2_add_relu_bwd<false>("tok_bn2_add_relu_bwd", gy, nullptr, y, x, mean, invstd, weight,
+                                 xd, mean_d, invstd_d, weight_d, dz, dx, grad_weight, grad_bias,
+                                 dxd, grad_weight_d, grad_bias_d, rows, channels, workspace,
+                                 cuda_stream);
+}
+
+extern "C" int tok_bn2_add_relu_bwd2(const void* gy, const void* gy2, const void* y, const void* x,
+                                     const float* mean, const float* invstd, const void* weight,
+                                     const void* xd, const float* mean_d, const float* invstd_d,
+                                     const void* weight_d, void* dz, void* dx, void* grad_weight,
+                                     void* grad_bias, void* dxd, void* grad_weight_d,
+                                     void* grad_bias_d, int64_t rows, int channels,
+                                     void* workspace, void* cuda_stream) {
+  return bn2_add_relu_bwd<true>("tok_bn2_add_relu_bwd2", gy, gy2, y, x, mean, invstd, weight, xd,
+                                mean_d, invstd_d, weight_d, dz, dx, grad_weight, grad_bias, dxd,
+                                grad_weight_d, grad_bias_d, rows, channels, workspace, cuda_stream);
 }

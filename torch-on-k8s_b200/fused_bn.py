@@ -26,6 +26,17 @@ channels_last-contiguous and 16-byte aligned like x, e.g. the zero-stride gy of 
 the stock backward: `threshold_backward` on the output (recomputed for bn_relu), then
 `native_batch_norm_backward` with the saved mean and invstd.
 
+    bn_add_relu(x, bn, r, shortcut=True)          == (y, y)
+    bn2_add_relu(x, bn, xd, bnd, shortcut=True)   == (y, y)
+
+fork a residual block's output for its two consumers, the next block's conv1 and its shortcut.
+Fused, the second is a view of y from the same autograd node, so the node receives the two
+consumers' gradients separately rather than autograd's sum of them; the reduction kernel adds them
+per element as that sum would (bf16(f(g1) + f(g2))), which saves the add's pass over both and its
+write and re-read of the sum.  When either gradient is one the kernels cannot read, the two are
+added as autograd would have added them and the backward goes on as for one gradient.  On the stock
+path the pair is (y, y), and autograd adds as it always does.
+
 The fused path is taken when the inputs allow it: CUDA, bf16 activations and batch-norm tensors,
 channels_last-contiguous 4-D activations with C % 8 == 0 and 16-byte aligned data, a module in
 training mode that tracks running statistics with a fixed momentum and a positive eps.  Anything
@@ -109,7 +120,7 @@ class _BnAddRelu(torch.autograd.Function):
     """y = relu(bn(x) [+ r | + bnd(xd)]); the residual is `r` (mode 1) or `xd` through `bnd` (mode 2)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, other, weight_d, bias_d, bn, bnd, mode):
+    def forward(ctx, x, weight, bias, other, weight_d, bias_d, bn, bnd, mode, shortcut):
         rows, ch = x.numel() // x.shape[1], x.shape[1]
         mean, var = _stats(x, bn)
         invstd = torch.empty_like(mean)
@@ -143,11 +154,15 @@ class _BnAddRelu(torch.autograd.Function):
             ctx.save_for_backward(x, mean, invstd, y, weight)
         else:
             ctx.save_for_backward(x, mean, invstd, other, mean_d, invstd_d, y, weight, weight_d)
+        if shortcut:
+            # an unused half arrives as None, not as a tensor of zeros
+            ctx.set_materialize_grads(False)
+            return y, y.view_as(y)
         return y
 
     @staticmethod
     @once_differentiable
-    def backward(ctx, gy):
+    def backward(ctx, gy, gy_short=None):
         need = ctx.needs_input_grad
         saved = ctx.saved_tensors
         x = saved[0]
@@ -156,6 +171,14 @@ class _BnAddRelu(torch.autograd.Function):
             if weight._version != vw or bias._version != vb:
                 raise RuntimeError("bn_relu: the batch norm's weight or bias was modified by an "
                                    "inplace operation after the forward")
+        if gy is not None and gy_short is not None and _same(x, gy) and _same(x, gy_short):
+            return _fused_backward(ctx, gy, need, saved, gy_short)
+        if gy_short is not None:
+            # autograd's sum, in its order: the shortcut's consumer comes later in the forward than
+            # the next conv1, so its gradient is the one autograd holds first
+            gy = gy_short if gy is None else gy_short + gy
+        if gy is None:
+            return (None,) * 10
         if _same(x, gy):
             return _fused_backward(ctx, gy, need, saved)
         if ctx.mode == 0:
@@ -180,12 +203,13 @@ class _BnAddRelu(torch.autograd.Function):
             dr = g
         dx, dw, db = _bn_backward(g, x, ctx.bn, mean, invstd, [need[0], need[1], need[2]])
         if ctx.mode == 2:
-            return dx, dw, db, dxd, dwd, dbd, None, None, None
-        return dx, dw, db, dr, None, None, None, None, None
+            return dx, dw, db, dxd, dwd, dbd, None, None, None, None
+        return dx, dw, db, dr, None, None, None, None, None, None
 
 
-def _fused_backward(ctx, gy, need, saved):
-    """threshold_backward + native_batch_norm_backward through libtok8s, for a gy laid out as x."""
+def _fused_backward(ctx, gy, need, saved, gy2=None):
+    """threshold_backward + native_batch_norm_backward through libtok8s, for a gy laid out as x;
+    with gy2 (modes 1, 2), of the gradient gy + gy2."""
     mode = ctx.mode
     x = saved[0]
     rows, ch = x.numel() // x.shape[1], x.shape[1]
@@ -216,9 +240,12 @@ def _fused_backward(ctx, gy, need, saved):
             _, mean, invstd, y, weight = saved
             dw, db = out(1, weight), out(2, weight)
             dz = torch.empty_like(x)
-            rc = lib.tok_bn_add_relu_bwd(_ptr(gy), _ptr(y), _ptr(x), _ptr(mean), _ptr(invstd),
-                                         _ptr(weight), _ptr(dz), ptr(dx), ptr(dw), ptr(db), rows, ch,
-                                         _ptr(work), stream)
+            tail = (_ptr(y), _ptr(x), _ptr(mean), _ptr(invstd), _ptr(weight), _ptr(dz), ptr(dx),
+                    ptr(dw), ptr(db), rows, ch, _ptr(work), stream)
+            if gy2 is None:
+                rc = lib.tok_bn_add_relu_bwd(_ptr(gy), *tail)
+            else:
+                rc = lib.tok_bn_add_relu_bwd2(_ptr(gy), _ptr(gy2), *tail)
             grads = (dx, dw, db, dz if need[3] else None)
         else:
             _, mean, invstd, xd, mean_d, invstd_d, y, weight, weight_d = saved
@@ -226,14 +253,17 @@ def _fused_backward(ctx, gy, need, saved):
             dxd = out(3, xd)
             dwd, dbd = out(4, weight_d), out(5, weight_d)
             dz = torch.empty_like(x)
-            rc = lib.tok_bn2_add_relu_bwd(_ptr(gy), _ptr(y), _ptr(x), _ptr(mean), _ptr(invstd),
-                                          _ptr(weight), _ptr(xd), _ptr(mean_d), _ptr(invstd_d),
-                                          _ptr(weight_d), _ptr(dz), ptr(dx), ptr(dw), ptr(db),
-                                          ptr(dxd), ptr(dwd), ptr(dbd), rows, ch, _ptr(work), stream)
+            tail = (_ptr(y), _ptr(x), _ptr(mean), _ptr(invstd), _ptr(weight), _ptr(xd), _ptr(mean_d),
+                    _ptr(invstd_d), _ptr(weight_d), _ptr(dz), ptr(dx), ptr(dw), ptr(db), ptr(dxd),
+                    ptr(dwd), ptr(dbd), rows, ch, _ptr(work), stream)
+            if gy2 is None:
+                rc = lib.tok_bn2_add_relu_bwd(_ptr(gy), *tail)
+            else:
+                rc = lib.tok_bn2_add_relu_bwd2(_ptr(gy), _ptr(gy2), *tail)
             _ffi.check(rc)
-            return dx, dw, db, dxd, dwd, dbd, None, None, None
+            return dx, dw, db, dxd, dwd, dbd, None, None, None, None
     _ffi.check(rc)
-    return grads + (None,) * 5
+    return grads + (None,) * 6
 
 
 def _stem_pool(pool: torch.nn.Module) -> bool:
@@ -289,20 +319,25 @@ def max_pool(x: torch.Tensor, pool: torch.nn.Module) -> torch.Tensor:
 def bn_relu(x: torch.Tensor, bn: torch.nn.Module) -> torch.Tensor:
     """relu(bn(x)), fused on CUDA bf16 channels_last training inputs."""
     if _fusable_act(x) and _fusable_bn(bn, x):
-        return _BnAddRelu.apply(x, bn.weight, bn.bias, None, None, None, bn, None, 0)
+        return _BnAddRelu.apply(x, bn.weight, bn.bias, None, None, None, bn, None, 0, False)
     return F.relu(bn(x), inplace=True)
 
 
-def bn_add_relu(x: torch.Tensor, bn: torch.nn.Module, r: torch.Tensor) -> torch.Tensor:
-    """relu(bn(x) + r), fused on CUDA bf16 channels_last training inputs."""
+def bn_add_relu(x: torch.Tensor, bn: torch.nn.Module, r: torch.Tensor, shortcut: bool = False):
+    """relu(bn(x) + r), fused on CUDA bf16 channels_last training inputs; with `shortcut`, the pair
+    (y, y) for two consumers whose gradients the fused backward sums in its reduction."""
     if _fusable_act(x) and _fusable_bn(bn, x) and _same(x, r):
-        return _BnAddRelu.apply(x, bn.weight, bn.bias, r, None, None, bn, None, 1)
-    return F.relu(bn(x) + r, inplace=True)
+        return _BnAddRelu.apply(x, bn.weight, bn.bias, r, None, None, bn, None, 1, shortcut)
+    y = F.relu(bn(x) + r, inplace=True)
+    return (y, y) if shortcut else y
 
 
-def bn2_add_relu(x: torch.Tensor, bn: torch.nn.Module, xd: torch.Tensor,
-                 bnd: torch.nn.Module) -> torch.Tensor:
-    """relu(bn(x) + bnd(xd)), fused on CUDA bf16 channels_last training inputs."""
+def bn2_add_relu(x: torch.Tensor, bn: torch.nn.Module, xd: torch.Tensor, bnd: torch.nn.Module,
+                 shortcut: bool = False):
+    """relu(bn(x) + bnd(xd)), fused on CUDA bf16 channels_last training inputs; with `shortcut`, the
+    pair (y, y) as bn_add_relu's."""
     if _fusable_act(x) and _fusable_bn(bn, x) and _same(x, xd) and _fusable_bn(bnd, xd):
-        return _BnAddRelu.apply(x, bn.weight, bn.bias, xd, bnd.weight, bnd.bias, bn, bnd, 2)
-    return F.relu(bn(x) + bnd(xd), inplace=True)
+        return _BnAddRelu.apply(x, bn.weight, bn.bias, xd, bnd.weight, bnd.bias, bn, bnd, 2,
+                                shortcut)
+    y = F.relu(bn(x) + bnd(xd), inplace=True)
+    return (y, y) if shortcut else y

@@ -5,7 +5,12 @@ network for checkpoints).
 Every batch norm is applied through torch_on_k8s_b200.fused_bn together with the ReLU and residual
 add that follow it: on CUDA bf16 channels_last training inputs that is one fused libtok8s kernel
 per site, bit-identical to the unfused ops; anything else runs the plain nn composition.  The stem's
-max pool runs through fused_bn.max_pool under the same conditions."""
+max pool runs through fused_bn.max_pool under the same conditions.
+
+A block hands its output to the next block as a pair (x, x_short), one for conv1 and one for the
+shortcut, so that the fused backward receives the two gradients separately and sums them inside its
+reduction instead of after an autograd add (fused_bn.bn_add_relu's `shortcut`).  The last block
+returns its output alone to the average pool."""
 from __future__ import annotations
 
 import torch
@@ -27,16 +32,18 @@ class Bottleneck(nn.Module):
         self.bn3 = nn.BatchNorm2d(planes * self.expansion)
         self.relu = nn.ReLU(inplace=True)
         self.downsample = downsample
+        self.fork = True  # return (y, y) for the next block's conv1 and shortcut
 
     def forward(self, x):
+        x, x_short = x if isinstance(x, tuple) else (x, x)
         out = bn_relu(self.conv1(x), self.bn1)
         out = bn_relu(self.conv2(out), self.bn2)
         out = self.conv3(out)
         if self.downsample is not None:
             # downsample = Sequential(conv, bn): its batch norm is fused into the residual add
             conv_d, bn_d = self.downsample
-            return bn2_add_relu(out, self.bn3, conv_d(x), bn_d)
-        return bn_add_relu(out, self.bn3, x)
+            return bn2_add_relu(out, self.bn3, conv_d(x_short), bn_d, shortcut=self.fork)
+        return bn_add_relu(out, self.bn3, x_short, shortcut=self.fork)
 
 
 class ResNet50(nn.Module):
@@ -51,6 +58,7 @@ class ResNet50(nn.Module):
         self.layer2 = self._make_layer(128, 4, 2)
         self.layer3 = self._make_layer(256, 6, 2)
         self.layer4 = self._make_layer(512, 3, 2)
+        self.layer4[-1].fork = False
         self.avgpool = nn.AdaptiveAvgPool2d((1, 1))
         self.fc = nn.Linear(512 * Bottleneck.expansion, num_classes)
         for m in self.modules():
