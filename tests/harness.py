@@ -27,6 +27,21 @@ if ROOT not in sys.path:
 NP2TOK = {"f32": 0, "bf16": 1, "f16": 2}
 
 
+class LibSpy:
+    """Stands in for the loaded libtok8s (monkeypatch _ffi.lib to return it) and records, in
+    `calls`, the name of every call to an entry point that starts with one of `prefixes`, except
+    those that end with one of `ignore`."""
+
+    def __init__(self, lib, prefixes, ignore=()):
+        self.lib, self.prefixes, self.ignore, self.calls = lib, tuple(prefixes), tuple(ignore), []
+
+    def __getattr__(self, name):
+        fn = getattr(self.lib, name)
+        if not name.startswith(self.prefixes) or (self.ignore and name.endswith(self.ignore)):
+            return fn
+        return lambda *a: self.calls.append(name) or fn(*a)
+
+
 def torch_dtype(name):
     import torch
     return {"f32": torch.float32, "bf16": torch.bfloat16, "f16": torch.float16}[name]

@@ -8,6 +8,7 @@
     tests, and the assertions the elastic tests share;
   * the C ABI refusal helpers and the gloo-DDP table check of the CPU suites.
 """
+import contextlib
 import hashlib
 import os
 import tempfile
@@ -361,6 +362,37 @@ def _reference(case, opt, params, masters, **kw):
                      clip=case["kw"].get("max_grad_norm"), **kw)
 
 
+@contextlib.contextmanager
+def captured_buckets(pidx, step_no, before=None, after=None):
+    """BucketAllreduceHook.__call__ wrapped so that every bucket is recorded before its exchange;
+    yields the list of records dict(step=step_no[0], index, pre (a clone of the bucket on the
+    compute stream), views [(pidx[parameter's data_ptr], element offset, numel, gradient
+    data_ptr)]).  before(bucket, record) runs before the real call, after(bucket, record) after it."""
+    from torch_on_k8s_b200 import ddp_hook
+    buckets = []
+    real_call = ddp_hook.BucketAllreduceHook.__call__
+
+    def traced(self, state, bucket):
+        buf = bucket.buffer()
+        pre = buf.clone()     # on the compute stream, before the exchange may touch the bucket
+        esz = buf.element_size()
+        views = [(pidx[p.data_ptr()], (g.data_ptr() - buf.data_ptr()) // esz, g.numel(), g.data_ptr())
+                 for p, g in zip(bucket.parameters(), bucket.gradients())]
+        b = dict(step=step_no[0], index=bucket.index(), pre=pre, views=views)
+        if before is not None:
+            before(bucket, b)
+        fut = real_call(self, state, bucket)
+        if after is not None:
+            after(bucket, b)
+        buckets.append(b)
+        return fut
+    ddp_hook.BucketAllreduceHook.__call__ = traced
+    try:
+        yield buckets
+    finally:
+        ddp_hook.BucketAllreduceHook.__call__ = real_call
+
+
 def ddp_replica(rank, world, device, path, cases, job):
     """One replica of a DDP run through Replica.wrap(optimizer=...) over make_model("conv"), every
     replica starting from different weights.  Each bucket is captured before its exchange; after the
@@ -375,7 +407,6 @@ def ddp_replica(rank, world, device, path, cases, job):
     import torch.distributed as dist
     from oracle.allreduce_oracle import allreduce_oracle
     from test_training_paths_gpu import make_batch, make_model
-    from torch_on_k8s_b200 import ddp_hook
     from torch_on_k8s_b200.worker import init_replica
 
     case = cases[0]
@@ -392,109 +423,102 @@ def ddp_replica(rank, world, device, path, cases, job):
     opt, params, ls = _new_optimizer(case, model)
     pidx = {p.data_ptr(): i for i, p in enumerate(params)}
     sch = sched(opt) if case["sched"] else None
-    buckets = []
-    real_call = ddp_hook.BucketAllreduceHook.__call__
 
-    def traced(self, state, bucket):
-        buf = bucket.buffer()
-        pre = buf.clone()     # on the compute stream, before the exchange may touch the bucket
-        esz = buf.element_size()
-        views = [(pidx[p.data_ptr()], (g.data_ptr() - buf.data_ptr()) // esz, g.numel(), g.data_ptr())
-                 for p, g in zip(bucket.parameters(), bucket.gradients())]
-        b = dict(step=step_no[0], index=bucket.index(), pre=pre, views=views)
+    def before(bucket, b):
         if clip is not None:
             b.update(params=list(bucket.parameters()),
-                     stepped=[bits(opt.state[p]["master_param"]).clone() for p in bucket.parameters()])
-        fut = real_call(self, state, bucket)
+                     stepped=[bits(opt.state[p]["master_param"]).clone()
+                              for p in bucket.parameters()])
+
+    def after(bucket, b):
         if table is not None:
-            key = ("norm", "bucket", bucket.index(), str(buf.dtype)) if table == "norm" else \
+            key = ("norm", "bucket", bucket.index(), str(bucket.buffer().dtype)) \
+                if table == "norm" else \
                 ("bucket", bucket.index(), 0, int(table == "fresh" and step_no[0] == 0))
             b["table_grads"] = [r[0] for r in opt._tables[key][0]]
-        buckets.append(b)
-        return fut
-    ddp_hook.BucketAllreduceHook.__call__ = traced
     step_no = [0]
-    try:
-        ddp, hook = rep.wrap(model, bucket_cap_mb=1, optimizer=opt)
-        torch.cuda.synchronize()
-        init_p = [p.detach().clone(memory_format=torch.preserve_format) for p in params]
-        init_w = [opt.state[p]["master_param"].clone(memory_format=torch.preserve_format)
-                  for p in params]
-        uploads, norms, skipped, scales, untouched = [], [], [], [], True
-        for step in range(steps):
-            step_no[0] = step
-            x, y = make_batch("conv", rank, step, dev)
-            opt.zero_grad(set_to_none=False)
-            loss = torch.nn.functional.cross_entropy(ddp(x.to(half)).float(), y)
-            if step == case.get("overflow") and rank == world - 1:
-                loss = loss * 2.0 ** 40   # this rank's scaled gradients overflow f16 in backward
-            (ls.scale(loss) if ls is not None else loss).backward()
-            if clip is not None:
-                torch.cuda.synchronize()
-                # nothing is stepped before step(): the global norm does not exist yet
-                for b in buckets:
-                    if b["step"] == step:
-                        untouched &= all(torch.equal(bits(opt.state[p]["master_param"]), w)
-                                         for p, w in zip(b["params"], b["stepped"]))
-            opt.step()
-            if sch is not None:
-                sch.step()
+    with captured_buckets(pidx, step_no, before, after) as buckets:
+        try:
+            ddp, hook = rep.wrap(model, bucket_cap_mb=1, optimizer=opt)
             torch.cuda.synchronize()
-            rep.comm.status()
-            uploads.append(opt.table_uploads)
-            if clip is not None:
-                norms.append(bits(opt.grad_norm).item())
+            init_p = [p.detach().clone(memory_format=torch.preserve_format) for p in params]
+            init_w = [opt.state[p]["master_param"].clone(memory_format=torch.preserve_format)
+                      for p in params]
+            uploads, norms, skipped, scales, untouched = [], [], [], [], True
+            for step in range(steps):
+                step_no[0] = step
+                x, y = make_batch("conv", rank, step, dev)
+                opt.zero_grad(set_to_none=False)
+                loss = torch.nn.functional.cross_entropy(ddp(x.to(half)).float(), y)
+                if step == case.get("overflow") and rank == world - 1:
+                    loss = loss * 2.0 ** 40   # this rank's scaled gradients overflow f16 in backward
+                (ls.scale(loss) if ls is not None else loss).backward()
+                if clip is not None:
+                    torch.cuda.synchronize()
+                    # nothing is stepped before step(): the global norm does not exist yet
+                    for b in buckets:
+                        if b["step"] == step:
+                            untouched &= all(torch.equal(bits(opt.state[p]["master_param"]), w)
+                                             for p, w in zip(b["params"], b["stepped"]))
+                opt.step()
+                if sch is not None:
+                    sch.step()
+                torch.cuda.synchronize()
+                rep.comm.status()
+                uploads.append(opt.table_uploads)
+                if clip is not None:
+                    norms.append(bits(opt.grad_norm).item())
+                if ls is not None:
+                    skipped.append(opt.step_skipped)
+                    scales.append(bits(ls.scale_tensor).item())
+            in_buckets = len(opt._stepped) == 0 and any(k[0] == "bucket" for k in opt._tables) \
+                and not any(k[0] == "group" for k in opt._tables)
+            # every replica's pre-exchange slices, averaged by the oracle, feed the restatement
+            mine = [dict(step=b["step"], views=b["views"], pre=harness.from_torch(b["pre"], dt))
+                    for b in buckets]
+            everyone = [None] * world
+            dist.all_gather_object(everyone, mine)
+            ref = _reference(case, opt, init_p, init_w, with_sched=case["sched"],
+                             scale=case.get("loss_scale"))
+            ref_norms, ref_skipped, clipped = [], [], 0
+            for step in range(steps):
+                slices = {}
+                for r in range(world):
+                    for b in everyone[r]:
+                        if b["step"] == step:
+                            for pi, off, n, _ in b["views"]:
+                                slices.setdefault(pi, [None] * world)[r] = b["pre"][off:off + n]
+                assert sorted(slices) == list(range(len(params))), (step, sorted(slices))
+                grads = []
+                for pi, p in enumerate(params):
+                    avg = allreduce_oracle(slices[pi], dt, dt, dt, 1.0 / world)
+                    g = torch.empty_strided(p.shape, p.stride(), dtype=p.dtype, device=dev)
+                    g.as_strided((p.numel(),), (1,)).copy_(harness.to_torch(avg, dt, dev))
+                    grads.append(g)
+                total, found = ref.step(grads)
+                if clip is not None:
+                    ref_norms.append(bits(total).item())
+                    clipped += total.item() + 1e-6 > clip
+                if ls is not None:
+                    ref_skipped.append(bool(found.item()))
+            torch.cuda.synchronize()
+            check_against(opt, params, ref, "rank %d of %d" % (rank, world),
+                          **case.get("compare", {}))
+            assert norms == ref_norms, (norms, ref_norms)
+            assert skipped == ref_skipped, (skipped, ref_skipped)
             if ls is not None:
-                skipped.append(opt.step_skipped)
-                scales.append(bits(ls.scale_tensor).item())
-        in_buckets = len(opt._stepped) == 0 and any(k[0] == "bucket" for k in opt._tables) \
-            and not any(k[0] == "group" for k in opt._tables)
-        # every replica's pre-exchange slices, averaged by the oracle, feed the restatement
-        mine = [dict(step=b["step"], views=b["views"], pre=harness.from_torch(b["pre"], dt))
-                for b in buckets]
-        everyone = [None] * world
-        dist.all_gather_object(everyone, mine)
-        ref = _reference(case, opt, init_p, init_w, with_sched=case["sched"],
-                         scale=case.get("loss_scale"))
-        ref_norms, ref_skipped, clipped = [], [], 0
-        for step in range(steps):
-            slices = {}
-            for r in range(world):
-                for b in everyone[r]:
-                    if b["step"] == step:
-                        for pi, off, n, _ in b["views"]:
-                            slices.setdefault(pi, [None] * world)[r] = b["pre"][off:off + n]
-            assert sorted(slices) == list(range(len(params))), (step, sorted(slices))
-            grads = []
-            for pi, p in enumerate(params):
-                avg = allreduce_oracle(slices[pi], dt, dt, dt, 1.0 / world)
-                g = torch.empty_strided(p.shape, p.stride(), dtype=p.dtype, device=dev)
-                g.as_strided((p.numel(),), (1,)).copy_(harness.to_torch(avg, dt, dev))
-                grads.append(g)
-            total, found = ref.step(grads)
-            if clip is not None:
-                ref_norms.append(bits(total).item())
-                clipped += total.item() + 1e-6 > clip
-            if ls is not None:
-                ref_skipped.append(bool(found.item()))
-        torch.cuda.synchronize()
-        check_against(opt, params, ref, "rank %d of %d" % (rank, world), **case.get("compare", {}))
-        assert norms == ref_norms, (norms, ref_norms)
-        assert skipped == ref_skipped, (skipped, ref_skipped)
-        if ls is not None:
-            assert same_bits(ls.scale_tensor, ref.scaler._scale)
-            assert same_bits(ls.growth_tracker, ref.scaler._growth_tracker)
-        layout = {s: sorted((b["index"], tuple(v[3] for v in b["views"])) for b in buckets
-                            if b["step"] == s) for s in range(steps)}
-        return dict(state=state_digests(opt, params, case["keys"], ls is not None),
-                    uploads=uploads, in_buckets=in_buckets, untouched=untouched,
-                    tables_ok=None if table is None else
-                    all(b["table_grads"] == [v[3] for v in b["views"]] for b in buckets),
-                    rebuilt=layout[0] != layout[1], stable=layout[1] == layout[steps - 1],
-                    norms=norms, clipped=clipped, skipped=skipped, scales=scales)
-    finally:
-        ddp_hook.BucketAllreduceHook.__call__ = real_call
-        rep.close()
+                assert same_bits(ls.scale_tensor, ref.scaler._scale)
+                assert same_bits(ls.growth_tracker, ref.scaler._growth_tracker)
+            layout = {s: sorted((b["index"], tuple(v[3] for v in b["views"])) for b in buckets
+                                if b["step"] == s) for s in range(steps)}
+            return dict(state=state_digests(opt, params, case["keys"], ls is not None),
+                        uploads=uploads, in_buckets=in_buckets, untouched=untouched,
+                        tables_ok=None if table is None else
+                        all(b["table_grads"] == [v[3] for v in b["views"]] for b in buckets),
+                        rebuilt=layout[0] != layout[1], stable=layout[1] == layout[steps - 1],
+                        norms=norms, clipped=clipped, skipped=skipped, scales=scales)
+        finally:
+            rep.close()
 
 
 def elastic_replica(proc, world, device, path, cases, job):

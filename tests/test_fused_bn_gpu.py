@@ -9,6 +9,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+import harness
+
 pytestmark = pytest.mark.gpu
 
 BF = torch.bfloat16
@@ -154,23 +156,10 @@ def test_saved_invstd_matches_native_batch_norm():
     assert_bits(invstd, sinv, "save_invstd")
 
 
-class Spy:
-    """Stands in for the loaded library and records the batch-norm calls."""
-
-    def __init__(self, lib):
-        self.lib, self.calls = lib, []
-
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if not name.startswith("tok_bn"):
-            return fn
-        return lambda *a: self.calls.append(name) or fn(*a)
-
-
 @pytest.fixture
 def spy(monkeypatch):
     from torch_on_k8s_b200 import _ffi
-    s = Spy(_ffi.lib())
+    s = harness.LibSpy(_ffi.lib(), ("tok_bn",))
     monkeypatch.setattr(_ffi, "lib", lambda: s)
     return s
 

@@ -12,6 +12,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+import harness
+
 pytestmark = pytest.mark.gpu
 
 BF = torch.bfloat16
@@ -198,23 +200,10 @@ def test_gradient_that_needs_a_layout_copy():
     assert_bits(xo.grad, xs.grad, "y.sum() gy")
 
 
-class Spy:
-    """Stands in for the loaded library and counts the max-pool calls."""
-
-    def __init__(self, lib):
-        self.lib, self.calls = lib, []
-
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if not name.startswith("tok_max_pool"):
-            return fn
-        return lambda *a: self.calls.append(name) or fn(*a)
-
-
 @pytest.fixture
 def spy(monkeypatch):
     from torch_on_k8s_b200 import _ffi
-    s = Spy(_ffi.lib())
+    s = harness.LibSpy(_ffi.lib(), ("tok_max_pool",))
     monkeypatch.setattr(_ffi, "lib", lambda: s)
     return s
 

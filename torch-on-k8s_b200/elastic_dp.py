@@ -76,7 +76,9 @@ class ElasticDataParallel(torch.nn.Module):
             flat.zero_()
             off = 0
             for p in ps:
-                p.grad = flat[off:off + p.numel()].view(p.shape)
+                # laid out in the bucket as the parameter is in memory (channels_last too), as DDP's
+                # gradient_as_bucket_view does: the master-weight optimizers refuse other strides
+                p.grad = flat[off:off + p.numel()].as_strided(p.shape, p.stride())
                 off += (p.numel() + 7) // 8 * 8
             self.buckets.append(flat)
             self.bucket_params.append(ps)
