@@ -481,6 +481,27 @@ int tok_lars_master_step(const tok_lars_segment_t* segments, int count, int64_t 
                          float* partials, const float* inv_scale, const float* grad_coef,
                          void* cuda_stream);
 
+/* Exponential moving average of fp32 master weights (torch_on_k8s_b200/optim.py's ema_decay), one
+ * launch per gradient bucket.  For every element of every segment it produces the bits of
+ * torch.optim.swa_utils.AveragedModel(..., multi_avg_fn=get_ema_multi_avg_fn(decay)).update_parameters
+ * on the masters: with `copy` != 0, ema = master (the first update, n_averaged == 0); otherwise
+ *   torch._foreach_lerp_(ema, masters, 1 - decay)
+ * with the weight formed as Python forms it, in double, and rounded to float once as ATen rounds the
+ * Scalar.  The table follows tok_sgd_master_step's rules (TOK_SGD_CHUNK elements per chunk, one CTA
+ * per chunk, a DEVICE array).  Segments may start at any element; 16-byte loads and stores are used
+ * where master and ema share an alignment phase, scalar ones otherwise; nothing outside the segments
+ * is read or written.  Returns TOK_ERR_INVALID for a null or empty table, a negative, zero or too
+ * large `chunks`, a decay that is NaN or outside [0, 1], TOK_ERR_NO_DEVICE without a GPU.  Enqueued
+ * on `cuda_stream`, no synchronisation. */
+typedef struct tok_ema_segment {
+  const float* master; /* fp32[numel], read                                                       */
+  float* ema;          /* fp32[numel], read (unless copy) and written                             */
+  int64_t numel;
+  int64_t chunk0;      /* index of this segment's first chunk                                     */
+} tok_ema_segment_t;
+int tok_ema_master_update(const tok_ema_segment_t* segments, int count, int64_t chunks,
+                          double decay, int copy, void* cuda_stream);
+
 /* Which algorithm AUTO picks for `wire_bytes` on this communicator. */
 int tok_allreduce_algo(tok_comm_t* comm, size_t wire_bytes, int* algo);
 /* Number of kernels this communicator has launched so far (bench.py's gpu_launches): exchange,

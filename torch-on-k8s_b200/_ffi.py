@@ -148,6 +148,7 @@ PROTOTYPES = {
     "tok_lars_master_step": (C.c_int, [_P, C.c_int, C.c_int64, C.c_int, C.c_double, C.c_double,
                                        C.c_double, C.c_double, C.c_int, C.c_int, C.c_double,
                                        C.c_int, C.c_double, _P, _P, _P, _P]),
+    "tok_ema_master_update": (C.c_int, [_P, C.c_int, C.c_int64, C.c_double, C.c_int, _P]),
     "tok_allreduce_algo": (C.c_int, [_P, C.c_size_t, _IP]),
     "tok_comm_launches": (C.c_int, [_P, C.POINTER(C.c_uint64)]),
     "tok_comm_symm_alloc": (C.c_int, [_P, C.c_size_t, _PP]),

@@ -111,13 +111,15 @@ class ElasticDataParallel(torch.nn.Module):
 
     def hand_over(self, optimizer: torch.optim.Optimizer, step: int, root: int = 0) -> int:
         """What every member runs right after a re-form or a join, before its next step: `root`'s
-        parameters, buffers, optimizer state, loss scale (when the optimizer has one) and step
-        counter to the whole group, in this order on every replica, then a device synchronize.
-        Returns `root`'s step."""
+        parameters, buffers, optimizer state, loss scale and moving-average counters (when the
+        optimizer has them) and step counter to the whole group, in this order on every replica, then
+        a device synchronize.  Returns `root`'s step."""
         self.sync_params(root)
         self.sync_optimizer_state(optimizer, root)
         if getattr(optimizer, "loss_scale", None) is not None:
             self.sync_loss_scale(optimizer.loss_scale, root)
+        if getattr(optimizer, "ema_decay", None) is not None:
+            self.sync_ema_counters(optimizer, root)
         cell = torch.zeros(2, dtype=torch.int64, device=next(self.module.parameters()).device)
         cell[0] = step
         self.comm.broadcast(cell, root)
@@ -146,6 +148,16 @@ class ElasticDataParallel(torch.nn.Module):
         loss_scale._refresh()
 
     @torch.no_grad()
+    def sync_ema_counters(self, optimizer, root: int = 0) -> None:
+        """Replicate `root`'s moving-average counters (ema_updates, ema_steps; one 16-byte
+        broadcast).  Without them a joiner would copy its masters into the average on its first
+        update, or update on other iterations than the rest of the group."""
+        cell = torch.tensor([optimizer.ema_updates, optimizer.ema_steps], dtype=torch.int64,
+                            device=next(self.module.parameters()).device)
+        self.comm.broadcast(cell, root)
+        optimizer.ema_updates, optimizer.ema_steps = cell.tolist()
+
+    @torch.no_grad()
     def sync_optimizer_state(self, optimizer: torch.optim.Optimizer, root: int = 0) -> None:
         """Replicate `root`'s optimizer state (SGD momentum buffers, Adam moments and step counts).
         Without it a joiner would apply the same averaged gradients with different momentum and the
@@ -158,7 +170,7 @@ class ElasticDataParallel(torch.nn.Module):
         # layout = for every parameter, which tensor-valued state keys the root holds (bitmask over
         # the sorted union of known keys; python scalars such as `step` ints travel as f64)
         keys = ["momentum_buffer", "exp_avg", "exp_avg_sq", "max_exp_avg_sq", "step", "square_avg",
-                "acc_delta", "sum", "master_param"]
+                "acc_delta", "sum", "master_param", "ema_param"]
         layout = torch.zeros(len(params), dtype=torch.int64, device=dev)
         if me == root:
             for i, p in enumerate(params):

@@ -127,6 +127,7 @@ holds the same averaged gradients and so reaches the same verdict and the same s
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 from typing import Dict, Iterable, List, Optional, Tuple
@@ -291,6 +292,20 @@ class DynamicLossScale:
             self._refresh()
 
 
+def _check_ema(ema_decay, ema_every) -> Tuple[Optional[float], int]:
+    if ema_decay is not None:
+        if isinstance(ema_decay, bool) or not isinstance(ema_decay, (int, float)):
+            raise ValueError("ema_decay must be a number in [0, 1] or None, got %r" % (ema_decay,))
+        # get_ema_multi_avg_fn's check and message; NaN too, which it would let through
+        if not 0.0 <= ema_decay <= 1.0:
+            raise ValueError(f"Invalid decay value {ema_decay} provided. Please provide a value in "
+                             "[0,1] range.")
+        ema_decay = float(ema_decay)
+    if isinstance(ema_every, bool) or not isinstance(ema_every, int) or ema_every < 1:
+        raise ValueError("ema_every must be an int >= 1, got %r" % (ema_every,))
+    return ema_decay, ema_every
+
+
 def _check_loss_scale(loss_scale) -> Optional[DynamicLossScale]:
     if loss_scale is not None and not isinstance(loss_scale, DynamicLossScale):
         raise TypeError("loss_scale must be a DynamicLossScale or None, got %s"
@@ -300,9 +315,22 @@ def _check_loss_scale(loss_scale) -> Optional[DynamicLossScale]:
 
 class _MasterWeightOptimizer(torch.optim.Optimizer):
     """What the master-weight optimizers share: the parameter checks, fp32 masters, the fp32 restore
-    of state_dict, bucket and whole-group stepping with the stream ordering, and the device tables
-    (uploaded once per launch layout).  A subclass says how one (bucket or group, param group) splits
-    into launches (_split) and launches one (_kernel)."""
+    of state_dict, bucket and whole-group stepping with the stream ordering, the device tables
+    (uploaded once per launch layout) and the moving average of the masters.  A subclass says how one
+    (bucket or group, param group) splits into launches (_split) and launches one (_kernel).
+
+    With `ema_decay=d`, every parameter also keeps `state[p]["ema_param"]`, an fp32 exponential moving
+    average of its master, created as a copy of the master.  Every `ema_every`-th step() call (the
+    first included) updates it after the step, skipped or not, with the bits of
+
+        avg = AveragedModel(masters, multi_avg_fn=get_ema_multi_avg_fn(d), use_buffers=False)
+        avg.update_parameters(masters)   # the first update copies, later ones lerp by 1 - d
+
+    over every parameter the optimizer holds, gradient or not (tok_ema_master_update).  Overlapped
+    without clipping or loss scaling, each bucket's update is enqueued behind its step on the exchange
+    stream; otherwise, and for what no bucket covered, step() enqueues it at its end.  `ema_updates`
+    (AveragedModel's n_averaged) and `ema_steps` (step() calls so far) are host ints that state_dict
+    carries; ema_weights() evaluates with the averages."""
 
     _FP32_STATE: Tuple[str, ...] = ("master_param",)   # state restored to fp32 by load_state_dict
     _CPU_STEP = False                                    # load_state_dict gives `step` a CPU float32
@@ -310,7 +338,8 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
     _CHUNK = CHUNK                                       # elements per chunk of the step's table
 
     def __init__(self, params, defaults: dict, max_grad_norm: Optional[float] = None,
-                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
+                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None,
+                 ema_decay: Optional[float] = None, ema_every: int = 1):
         self._group_of: Dict[int, int] = {}          # id(param) -> index of its param group
         self._slot_of: Dict[int, int] = {}           # id(param) -> position in param-group order
         self._tables: Dict[tuple, tuple] = {}        # launch key -> (rows, device table)
@@ -326,6 +355,10 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         self.found_inf: Optional[torch.Tensor] = None   # loss scaling: the last step's verdict
         self.step_skipped = False                        # loss scaling: the last step was skipped
         self._found_inf: Optional[torch.Tensor] = None  # loss scaling: this iteration's verdict
+        self.ema_decay, self.ema_every = _check_ema(ema_decay, ema_every)
+        self.ema_updates = 0                             # EMA: AveragedModel's n_averaged
+        self.ema_steps = 0                               # EMA: step() calls so far
+        self._averaged: set = set()                      # EMA: id(param) averaged by a bucket
         self.table_uploads = 0
         super().__init__(params, defaults)
 
@@ -349,8 +382,11 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         for p in group["params"]:
             self._group_of[id(p)] = len(self.param_groups) - 1
             self._slot_of[id(p)] = len(self._slot_of)
-            self.state[p]["master_param"] = p.detach().to(torch.float32, copy=True,
-                                                          memory_format=torch.preserve_format)
+            st = self.state[p]
+            st["master_param"] = p.detach().to(torch.float32, copy=True,
+                                               memory_format=torch.preserve_format)
+            if self.ema_decay is not None:   # AveragedModel's deep copy at construction
+                st["ema_param"] = st["master_param"].clone(memory_format=torch.preserve_format)
 
     def load_state_dict(self, state_dict: dict) -> None:
         # Optimizer.load_state_dict casts floating state to the parameter's dtype: restore fp32, and a
@@ -359,12 +395,26 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         params = [p for g in self.param_groups for p in g["params"]]
         for i, saved in state_dict["state"].items():
             p = params[i]
-            for k in self._FP32_STATE:
+            for k in self._FP32_STATE + ("ema_param",):
                 if k in saved:
                     self.state[p][k] = saved[k].to(device=p.device, dtype=torch.float32, copy=True)
             if self._CPU_STEP and "step" in saved:
                 self.state[p]["step"] = torch.as_tensor(saved["step"]).to("cpu", torch.float32,
                                                                           copy=True)
+        if self.ema_decay is not None:
+            # a checkpoint without an average starts one: its first update copies the masters
+            self.ema_updates = int(state_dict.get("ema_updates", 0))
+            self.ema_steps = int(state_dict.get("ema_steps", 0))
+            for p in params:
+                st = self.state[p]
+                if "ema_param" not in st:
+                    st["ema_param"] = st["master_param"].clone(memory_format=torch.preserve_format)
+
+    def state_dict(self) -> dict:
+        out = super().state_dict()
+        if self.ema_decay is not None:
+            out["ema_updates"], out["ema_steps"] = self.ema_updates, self.ema_steps
+        return out
 
     # ---- stepping ------------------------------------------------------------------------------
     def _split(self, group: dict, pairs) -> List[tuple]:
@@ -490,19 +540,68 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
         self.found_inf = found_inf
         self._found_inf = torch.zeros((), dtype=torch.float32, device=found_inf.device)
 
+    # ---- moving average ----------------------------------------------------------------------------
+    def _ema_due(self) -> bool:
+        """This iteration updates the average: AveragedModel.update_parameters every ema_every-th
+        step() call, from the first."""
+        return self.ema_decay is not None and self.ema_steps % self.ema_every == 0
+
+    def _ema_entries(self, params) -> List[tuple]:
+        """[(master, ema)] of `params`: segment_table gives tok_ema_segment_t rows for them."""
+        return [(self.state[p]["master_param"], self.state[p]["ema_param"]) for p in params]
+
+    def _average(self, params, key: tuple, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Enqueue the update of the averages of `params` (on one device) on `stream` (which must
+        then be current) or the current stream."""
+        if not params[0].is_cuda:
+            raise RuntimeError("%s averages CUDA parameters only: the kernel has no CPU fallback"
+                               % type(self).__name__)
+        stream = stream or torch.cuda.current_stream(params[0].device)
+        rows, chunks = segment_table(self._ema_entries(params))
+        self._averaged.update(id(p) for p in params)
+        if not chunks:
+            return
+        table = self._table(key, rows, params[0].device)
+        with torch.cuda.device(params[0].device):
+            _ffi.check(_ffi.lib().tok_ema_master_update(
+                C.c_void_p(table.data_ptr()), len(rows), chunks, self.ema_decay,
+                int(self.ema_updates == 0), C.c_void_p(stream.cuda_stream)))
+
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """Evaluate with the averages: inside the context every parameter holds RNE(ema_param), the
+        bf16 / f16 weights of the averaged model; on exit it holds RNE(master) again, which it held
+        before (the restore is exact).  Buffers are not averaged (AveragedModel's
+        use_buffers=False): batch norm evaluates with the live model's running statistics."""
+        if self.ema_decay is None:
+            raise RuntimeError("%s keeps no moving average: pass ema_decay=" % type(self).__name__)
+        params = [p for g in self.param_groups for p in g["params"]]
+        with torch.no_grad():
+            for p in params:
+                p.copy_(self.state[p]["ema_param"])
+        try:
+            yield
+        finally:
+            with torch.no_grad():
+                for p in params:
+                    p.copy_(self.state[p]["master_param"])
+
     # ---- stepping paths --------------------------------------------------------------------------
     def _enqueue(self, by_group: Dict[int, list], where: tuple,
                  stream: Optional[torch.cuda.Stream] = None) -> None:
         """Take [(param, grad)] per param group index, of gradient bucket `index` (`where` is
         ("bucket", index)) or of what no bucket covered (("group",)), on `stream` or the current
-        stream.  Without max_grad_norm or a loss scale, step them; otherwise enqueue their vote and
-        keep them for _finish."""
+        stream.  Without max_grad_norm or a loss scale, step them, and update a bucket's averages
+        behind its step when this iteration updates them; otherwise enqueue their vote and keep them
+        for _finish."""
         pairs = [pg for prs in by_group.values() for pg in prs]
         self._check_pairs(pairs)
         with torch.cuda.stream(stream):
             if self.max_grad_norm is None and self.loss_scale is None:
                 for gi, prs in by_group.items():
                     self._launch(self.param_groups[gi], prs, where + (gi,), stream)
+                if where[0] == "bucket" and self._ema_due():
+                    self._average([p for p, _ in pairs], ("ema",) + where, stream)
             else:
                 dev = pairs[0][0].device
                 self._vote(pairs, where, dev, stream or torch.cuda.current_stream(dev))
@@ -599,10 +698,23 @@ class _MasterWeightOptimizer(torch.optim.Optimizer):
                 self._enqueue(rest, ("group",))
             if self.max_grad_norm is not None or self.loss_scale is not None:
                 self._finish()
+            if self._ema_due():
+                # after every step, skipped ones included: what no bucket averaged, one launch per
+                # device
+                by_dev: Dict[torch.device, list] = {}
+                for group in self.param_groups:
+                    for p in group["params"]:
+                        if id(p) not in self._averaged:
+                            by_dev.setdefault(p.device, []).append(p)
+                for dev, ps in by_dev.items():
+                    self._average(ps, ("ema", "rest", str(dev)))
+                self.ema_updates += 1
+            self.ema_steps += 1
         finally:
             self._stepped.clear()
             self._streams.clear()
             self._pending.clear()
+            self._averaged.clear()
         return loss
 
 
@@ -660,13 +772,14 @@ class MasterWeightSGD(_MasterWeightOptimizer):
     def __init__(self, params, lr: float, momentum: float = 0.0, dampening: float = 0.0,
                  weight_decay: float = 0.0, nesterov: bool = False, *, maximize: bool = False,
                  differentiable: bool = False, max_grad_norm: Optional[float] = None,
-                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
+                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None,
+                 ema_decay: Optional[float] = None, ema_every: int = 1):
         _check_sgd_args(lr, momentum, dampening, weight_decay, nesterov)
         if maximize or differentiable:
             raise ValueError("MasterWeightSGD supports neither maximize nor differentiable")
         super().__init__(params, dict(lr=lr, momentum=momentum, dampening=dampening,
                                       weight_decay=weight_decay, nesterov=nesterov),
-                         max_grad_norm, error_if_nonfinite, loss_scale)
+                         max_grad_norm, error_if_nonfinite, loss_scale, ema_decay, ema_every)
 
     def _split(self, group: dict, pairs) -> List[tuple]:
         """One launch per momentum state: fresh buffers (subkey 1), then the rest (subkey 0)."""
@@ -698,7 +811,8 @@ class MasterWeightAdam(_MasterWeightOptimizer):
                  foreach: Optional[bool] = None, maximize: bool = False, capturable: bool = False,
                  differentiable: bool = False, fused: Optional[bool] = None,
                  decoupled_weight_decay: bool = False, max_grad_norm: Optional[float] = None,
-                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
+                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None,
+                 ema_decay: Optional[float] = None, ema_every: int = 1):
         name = type(self).__name__
         if isinstance(lr, torch.Tensor) or any(isinstance(b, torch.Tensor) for b in betas):
             raise ValueError("%s takes lr and betas as Python floats, not Tensors" % name)
@@ -709,7 +823,7 @@ class MasterWeightAdam(_MasterWeightOptimizer):
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay,
                                       amsgrad=amsgrad,
                                       decoupled_weight_decay=decoupled_weight_decay),
-                         max_grad_norm, error_if_nonfinite, loss_scale)
+                         max_grad_norm, error_if_nonfinite, loss_scale, ema_decay, ema_every)
 
     def _split(self, group: dict, pairs) -> List[tuple]:
         return _split_by_step(self, pairs, group["amsgrad"])
@@ -733,11 +847,13 @@ class MasterWeightAdamW(MasterWeightAdam):
                  maximize: bool = False, foreach: Optional[bool] = None, capturable: bool = False,
                  differentiable: bool = False, fused: Optional[bool] = None,
                  max_grad_norm: Optional[float] = None, error_if_nonfinite: bool = False,
-                 loss_scale: Optional[DynamicLossScale] = None):
+                 loss_scale: Optional[DynamicLossScale] = None, ema_decay: Optional[float] = None,
+                 ema_every: int = 1):
         super().__init__(params, lr, betas, eps, weight_decay, amsgrad, foreach=foreach,
                          maximize=maximize, capturable=capturable, differentiable=differentiable,
                          fused=fused, decoupled_weight_decay=True, max_grad_norm=max_grad_norm,
-                         error_if_nonfinite=error_if_nonfinite, loss_scale=loss_scale)
+                         error_if_nonfinite=error_if_nonfinite, loss_scale=loss_scale,
+                         ema_decay=ema_decay, ema_every=ema_every)
 
 
 class MasterWeightLAMB(_MasterWeightOptimizer):
@@ -755,7 +871,8 @@ class MasterWeightLAMB(_MasterWeightOptimizer):
                  eps: float = 1e-6, weight_decay: float = 1e-2, amsgrad: bool = False, *,
                  maximize: bool = False, capturable: bool = False, differentiable: bool = False,
                  fused: Optional[bool] = None, max_grad_norm: Optional[float] = None,
-                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None):
+                 error_if_nonfinite: bool = False, loss_scale: Optional[DynamicLossScale] = None,
+                 ema_decay: Optional[float] = None, ema_every: int = 1):
         name = type(self).__name__
         if isinstance(lr, torch.Tensor) or any(isinstance(b, torch.Tensor) for b in betas):
             raise ValueError("%s takes lr and betas as Python floats, not Tensors" % name)
@@ -764,7 +881,7 @@ class MasterWeightLAMB(_MasterWeightOptimizer):
                              "fused" % name)
         _check_adam_args(lr, betas, eps, weight_decay)
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay),
-                         max_grad_norm, error_if_nonfinite, loss_scale)
+                         max_grad_norm, error_if_nonfinite, loss_scale, ema_decay, ema_every)
 
     def _split(self, group: dict, pairs) -> List[tuple]:
         """Adam's: one launch per (step count, dtype), entries without max_exp_avg_sq."""
@@ -820,12 +937,14 @@ class MasterWeightLARS(_MasterWeightOptimizer):
                  weight_decay: float = 0.0, nesterov: bool = False, *,
                  trust_coefficient: float = 0.02, clip: bool = True, eps: float = 1e-8,
                  max_grad_norm: Optional[float] = None, error_if_nonfinite: bool = False,
-                 loss_scale: Optional[DynamicLossScale] = None):
+                 loss_scale: Optional[DynamicLossScale] = None, ema_decay: Optional[float] = None,
+                 ema_every: int = 1):
         defaults = dict(lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay,
                         nesterov=nesterov, trust_coefficient=trust_coefficient, clip=clip, eps=eps,
                         lars=True)
         _check_lars_group(defaults)
-        super().__init__(params, defaults, max_grad_norm, error_if_nonfinite, loss_scale)
+        super().__init__(params, defaults, max_grad_norm, error_if_nonfinite, loss_scale,
+                         ema_decay, ema_every)
 
     _check_group = staticmethod(_check_lars_group)
 

@@ -59,8 +59,11 @@ class Replica:
         if self.world > 1 and not ddp_kwargs["init_sync"]:
             self.broadcast_module_states(model)
         if self.world > 1 and optimizer is not None:   # the masters follow rank 0's parameters
-            self.comm.broadcast_coalesced([optimizer.state[p]["master_param"]
-                                           for g in optimizer.param_groups for p in g["params"]], 0)
+            # and so do the moving averages, copies of the masters until the first step
+            self.comm.broadcast_coalesced([optimizer.state[p][k]
+                                           for g in optimizer.param_groups for p in g["params"]
+                                           for k in ("master_param", "ema_param")
+                                           if k in optimizer.state[p]], 0)
         scope = self.comm.symmetric if pooled else contextlib.nullcontext
         with scope():
             ddp = DDP(model, device_ids=[self.device.index], bucket_cap_mb=bucket_cap_mb,

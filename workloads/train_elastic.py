@@ -80,9 +80,16 @@ def main() -> int:
     ap.add_argument("--loss-scale", action="store_true",
                     help="dynamic loss scaling with torch.amp.GradScaler's defaults "
                          "(torch_on_k8s_b200.optim.DynamicLossScale); needs --master-weights")
+    ap.add_argument("--ema-decay", type=float, default=None, metavar="X",
+                    help="keep an exponential moving average of the fp32 master weights with decay "
+                         "X (AveragedModel with get_ema_multi_avg_fn(X)); needs --master-weights")
+    ap.add_argument("--ema-every", type=int, default=1, metavar="N",
+                    help="update the moving average every N steps (default 1)")
     a = ap.parse_args()
     if a.loss_scale and not a.master_weights:
         ap.error("--loss-scale needs --master-weights: stock GradScaler refuses f16 gradients")
+    if a.ema_decay is not None and not a.master_weights:
+        ap.error("--ema-decay needs --master-weights: it averages the fp32 masters")
     if a.optimizer in ("lamb", "lars") and not a.master_weights:
         ap.error("--optimizer %s needs --master-weights: torch.optim has no %s"
                  % (a.optimizer, a.optimizer.upper()))
@@ -110,18 +117,19 @@ def main() -> int:
                                              MasterWeightLARS, MasterWeightSGD,
                                              lamb_param_groups, lars_param_groups)
         ls = DynamicLossScale() if a.loss_scale else None
+        ema = dict(ema_decay=a.ema_decay, ema_every=a.ema_every)
         if a.optimizer == "lamb":
             opt = MasterWeightLAMB(lamb_param_groups(model.parameters()), lr=a.lr,
-                                   max_grad_norm=a.clip_grad_norm, loss_scale=ls)
+                                   max_grad_norm=a.clip_grad_norm, loss_scale=ls, **ema)
         elif a.optimizer == "lars":
             opt = MasterWeightLARS(lars_param_groups(model.parameters(), 5e-5), lr=a.lr,
-                                   momentum=0.9, max_grad_norm=a.clip_grad_norm, loss_scale=ls)
+                                   momentum=0.9, max_grad_norm=a.clip_grad_norm, loss_scale=ls, **ema)
         elif a.optimizer == "adamw":
             opt = MasterWeightAdamW(model.parameters(), lr=a.lr, max_grad_norm=a.clip_grad_norm,
-                                    loss_scale=ls)
+                                    loss_scale=ls, **ema)
         else:
             opt = MasterWeightSGD(model.parameters(), lr=a.lr, momentum=0.9,
-                                  max_grad_norm=a.clip_grad_norm, loss_scale=ls)
+                                  max_grad_norm=a.clip_grad_norm, loss_scale=ls, **ema)
     else:
         opt = torch.optim.AdamW(model.parameters(), lr=a.lr) if a.optimizer == "adamw" else \
             torch.optim.SGD(model.parameters(), lr=a.lr, momentum=0.9)
