@@ -166,8 +166,9 @@ __global__ void __launch_bounds__(kBnThreads) bn_fused_fwd_kernel(const BnArgs p
 //   finish    var = m2 / n (IEEE division)
 //   running   r_mean = bf16(fma(mean, momentum, (1 - momentum) * r_mean))
 //             r_var  = bf16(fma(var * bessel, momentum, (1 - momentum) * r_var))
-// The geometry is bn_stats_geom.h's.  Logical thread (by, ty) of ATen becomes one thread per 8-channel
-// vector here; its 4 chains visit rows p + (4i + j) * P (p = by * block_y + ty, P = block_y * grid_y).
+// The geometry is bn_stats_geom.h's.  Logical thread (by, ty) of ATen becomes 4 lanes per 8-channel
+// vector here; lane j runs chain j over rows p + (4i + j) * P (p = by * block_y + ty,
+// P = block_y * grid_y).
 struct StatsArgs {
   const uint4* x;
   int* ws_count;   // grid_y > 1: per logical block partials, merged by the finish kernel
@@ -188,11 +189,11 @@ struct StatsArgs {
 };
 
 constexpr int kStatsThreads = 256;  // physical threads per block of the finish kernel
-// Physical threads per block of the partial kernel.  At ~160 registers a thread, 128-thread blocks
-// let 3 blocks share an SM, and they split the 128 logical blocks of a 64-channel site over 128
-// SMs rather than fewer.
-constexpr int kStatsPartialThreads = 128;
-constexpr int kStatsDepth = 2;      // iterations (of 4 rows) loaded ahead of the one computed
+// Physical threads per block of the partial kernel, and chain steps loaded ahead of the one
+// computed.  At <= 64 registers two blocks share an SM: a 64-channel site's 128 logical blocks run
+// 16 warps on each SM, with 512 * 4 * 16 B = 32 KB of loads in flight.
+constexpr int kStatsPartialThreads = 512;
+constexpr int kStatsDepth = 4;
 
 // Folds (nb, mean_b, m2_b) into (n, mean, m2); the caller then adds nb to n (one count serves the
 // 8 channels of a vector).
@@ -219,116 +220,128 @@ __device__ __forceinline__ void stats_finish(const StatsArgs& a, int c, int n, f
       __float2bfloat16_rn(__fmaf_rn(__fmul_rn(var, a.bessel), a.momentum, __fmul_rn(keep, rv)));
 }
 
-__device__ __forceinline__ void load_rows(const StatsArgs& a, int v, int64_t row, int64_t stride,
-                                          uint4 (&q)[kStatsChains]) {
-#pragma unroll
-  for (int j = 0; j < kStatsChains; ++j) {
-    const int64_t r = row + j * stride;
-    q[j] = r < a.rows ? __ldg(a.x + r * a.vecs + v) : make_uint4(0, 0, 0, 0);
-  }
-}
-
-// blockDim = (tile, block_y): thread (vx, ty) of block (bx, by) owns vector bx * tile + vx of
-// logical thread (by, ty).
-__global__ void __launch_bounds__(kStatsPartialThreads) bn_stats_partial_kernel(const StatsArgs a) {
-  __shared__ float s_mean[kStatsPartialThreads][kVec];
-  __shared__ float s_m2[kStatsPartialThreads][kVec];
-  __shared__ int s_n[kStatsPartialThreads];
-  const int tile = blockDim.x, ty = threadIdx.y;
-  const int v = blockIdx.x * tile + threadIdx.x;
+// blockDim = (4 * tile, block_y): lane j = threadIdx.x % 4 of thread (vx = threadIdx.x / 4, ty) of
+// block (bx, by) runs chain j of logical thread (by, ty) on vector bx * tile + vx, the mapping of
+// bn_bwd_partial_kernel.
+__global__ void __launch_bounds__(kStatsPartialThreads, 2)
+    bn_stats_partial_kernel(const StatsArgs a) {
+  constexpr int kSlots = kStatsPartialThreads / kStatsChains;
+  __shared__ float s_mean[kSlots][kVec];
+  __shared__ float s_m2[kSlots][kVec];
+  __shared__ int s_n[kSlots];
+  const int j = threadIdx.x % kStatsChains, tile = blockDim.x / kStatsChains, ty = threadIdx.y;
+  const int vx = threadIdx.x / kStatsChains;
+  const int v = blockIdx.x * tile + vx;
   const bool live = v < a.vecs;
   const int64_t stride = (int64_t)a.block_y * a.grid_y;
-  const int64_t p = (int64_t)blockIdx.y * a.block_y + ty;
+  const int64_t step = kStatsChains * stride;
+  const int64_t p = (int64_t)blockIdx.y * a.block_y + ty + j * stride;
 
-  float mean[kStatsChains][kVec], m2[kStatsChains][kVec];
-  int n[kStatsChains];
+  float mean[kVec], m2[kVec];
+  int n = 0;
 #pragma unroll
-  for (int j = 0; j < kStatsChains; ++j) {
-    n[j] = 0;
-#pragma unroll
-    for (int k = 0; k < kVec; ++k) mean[j][k] = m2[j][k] = 0.0f;
-  }
+  for (int k = 0; k < kVec; ++k) mean[k] = m2[k] = 0.0f;
 
   if (live) {
-    uint4 buf[kStatsDepth][kStatsChains];
+    uint4 buf[kStatsDepth];
 #pragma unroll
-    for (int s = 0; s < kStatsDepth; ++s)
-      load_rows(a, v, p + (int64_t)s * kStatsChains * stride, stride, buf[s]);
+    for (int s = 0; s < kStatsDepth; ++s) {
+      const int64_t r = p + s * step;
+      buf[s] = r < a.rows ? __ldg(a.x + r * a.vecs + v) : make_uint4(0, 0, 0, 0);
+    }
     for (int i0 = 0; i0 < a.loop_count; i0 += kStatsDepth) {
 #pragma unroll
       for (int s = 0; s < kStatsDepth; ++s) {
+        // The buffer turns over whether or not step i runs (a load past the last iteration is past
+        // the last row, so it reads nothing): a conditional turnover would make the compiler copy
+        // the register a load is still filling, and wait for that load.
         const int i = i0 + s;
+        const int64_t row = p + (int64_t)i * step;
+        const uint4 q = buf[s];
+        const int64_t r = row + kStatsDepth * step;
+        buf[s] = r < a.rows ? __ldg(a.x + r * a.vecs + v) : make_uint4(0, 0, 0, 0);
         if (i < a.loop_count) {
-          const int64_t row = p + (int64_t)i * kStatsChains * stride;
-          uint4 next[kStatsChains];
-          load_rows(a, v, row + (int64_t)kStatsDepth * kStatsChains * stride, stride, next);
           // A chain's valid slots are a prefix of its iterations, so a valid slot of iteration i
-          // has count i + 1: one correctly rounded 1 / count serves 4 chains of 8 channels.
-          const float inv_i = __frcp_rn(__int2float_rn(i + 1));
+          // has count i + 1.
+          const bool valid = row < a.rows;
+          if (valid) ++n;
+          const float inv = valid ? __frcp_rn(__int2float_rn(i + 1)) : 0.0f;
+          const float vf = valid ? 1.0f : 0.0f;
 #pragma unroll
-          for (int j = 0; j < kStatsChains; ++j) {
-            const bool valid = row + j * stride < a.rows;
-            if (valid) ++n[j];
-            const float inv = valid ? inv_i : 0.0f;
-            const float vf = valid ? 1.0f : 0.0f;
-#pragma unroll
-            for (int k = 0; k < kVec; ++k) {
-              const float x = widen(word(buf[s][j], k >> 1), k & 1);
-              const float d0 = __fsub_rn(x, mean[j][k]);
-              mean[j][k] = __fmaf_rn(d0, inv, mean[j][k]);
-              const float d1 = __fsub_rn(x, mean[j][k]);
-              m2[j][k] = __fmaf_rn(__fmul_rn(d0, d1), vf, m2[j][k]);
-            }
-            buf[s][j] = next[j];
+          for (int k = 0; k < kVec; ++k) {
+            const float x = widen(word(q, k >> 1), k & 1);
+            const float d0 = __fsub_rn(x, mean[k]);
+            mean[k] = __fmaf_rn(d0, inv, mean[k]);
+            const float d1 = __fsub_rn(x, mean[k]);
+            m2[k] = __fmaf_rn(__fmul_rn(d0, d1), vf, m2[k]);
           }
         }
       }
     }
   }
 
+  // chains 1, 2, 3 into chain 0, in order
+  const int tid = threadIdx.y * blockDim.x + threadIdx.x;
+  const int nthreads = blockDim.x * blockDim.y;
+  const int lanes = min(32, nthreads - (tid & ~31));
+  const unsigned mask = lanes == 32 ? 0xffffffffu : (1u << lanes) - 1u;
+  // (every lane runs the merge on what it reads, so all reads of a value precede its update)
+  int nb[kStatsChains];
 #pragma unroll
-  for (int j = 1; j < kStatsChains; ++j) {
+  for (int c = 1; c < kStatsChains; ++c) nb[c] = __shfl_sync(mask, n, c, kStatsChains);
 #pragma unroll
-    for (int k = 0; k < kVec; ++k)
-      welford_merge<true>(n[0], mean[0][k], m2[0][k], n[j], mean[j][k], m2[j][k]);
-    n[0] += n[j];
+  for (int k = 0; k < kVec; ++k) {
+    float mean_b[kStatsChains], m2_b[kStatsChains];
+#pragma unroll
+    for (int c = 1; c < kStatsChains; ++c) {
+      mean_b[c] = __shfl_sync(mask, mean[k], c, kStatsChains);
+      m2_b[c] = __shfl_sync(mask, m2[k], c, kStatsChains);
+    }
+    int na = n;
+#pragma unroll
+    for (int c = 1; c < kStatsChains; ++c) {
+      welford_merge<true>(na, mean[k], m2[k], nb[c], mean_b[c], m2_b[c]);
+      na += nb[c];
+    }
   }
+#pragma unroll
+  for (int c = 1; c < kStatsChains; ++c) n += nb[c];
 
-  // ATen's welford_merge_block_vertical over ty
-  const int slot = ty * tile + threadIdx.x;
+  // ATen's welford_merge_block_vertical over ty, lane 0 of each chain group
+  const int slot = ty * tile + vx;
   for (int off = a.block_y / 2; off > 0; off >>= 1) {
-    if (ty < 2 * off) {
+    if (j == 0 && ty < 2 * off) {
 #pragma unroll
       for (int k = 0; k < kVec; ++k) {
-        s_mean[slot][k] = mean[0][k];
-        s_m2[slot][k] = m2[0][k];
+        s_mean[slot][k] = mean[k];
+        s_m2[slot][k] = m2[k];
       }
-      s_n[slot] = n[0];
+      s_n[slot] = n;
     }
     __syncthreads();
-    if (ty < off) {
+    if (j == 0 && ty < off) {
       const int o = slot + off * tile;
       const int nb = s_n[o];
 #pragma unroll
       for (int k = 0; k < kVec; ++k)
-        welford_merge<false>(n[0], mean[0][k], m2[0][k], nb, s_mean[o][k], s_m2[o][k]);
-      n[0] += nb;
+        welford_merge<false>(n, mean[k], m2[k], nb, s_mean[o][k], s_m2[o][k]);
+      n += nb;
     }
     __syncthreads();
   }
-  if (ty != 0 || !live) return;
+  if (j != 0 || ty != 0 || !live) return;
   if (a.grid_y == 1) {
 #pragma unroll
-    for (int k = 0; k < kVec; ++k) stats_finish(a, v * kVec + k, n[0], mean[0][k], m2[0][k]);
+    for (int k = 0; k < kVec; ++k) stats_finish(a, v * kVec + k, n, mean[k], m2[k]);
     return;
   }
   const int64_t base = (int64_t)blockIdx.y * a.channels + v * kVec;
 #pragma unroll
   for (int k = 0; k < kVec; ++k) {
-    a.ws_mean[base + k] = mean[0][k];
-    a.ws_m2[base + k] = m2[0][k];
+    a.ws_mean[base + k] = mean[k];
+    a.ws_m2[base + k] = m2[k];
   }
-  if (v == 0) a.ws_count[blockIdx.y] = n[0];
+  if (v == 0) a.ws_count[blockIdx.y] = n;
 }
 
 // ATen's last-block merge: blockDim = (kStatsThreads / block_y, block_y), one channel per column.
@@ -425,9 +438,10 @@ struct BwdArgs {
 };
 
 constexpr int kBwdPartialThreads = 512;  // physical threads per block of the reduction
-// chain steps loaded ahead of the one computed (mode 2 loads four streams a step, five with gy2)
+// chain steps loaded ahead of the one computed (mode 1 loads three streams a step, four with gy2;
+// mode 2 four, five with gy2): the most that fit 128 registers without spilling
 template <int kMode>
-constexpr int kBwdDepth = kMode == 2 ? 2 : 4;
+constexpr int kBwdDepth = kMode == 2 ? 2 : kMode == 1 ? 3 : 4;
 constexpr int kBwdStreams = 5;           // gy, x, y, xd, gy2
 
 __device__ __forceinline__ float relu_grad(float g, float v) { return v <= 0.0f ? 0.0f : g; }
@@ -506,12 +520,13 @@ __global__ void __launch_bounds__(kBwdPartialThreads) bn_bwd_partial_kernel(cons
     for (int i0 = 0; i0 < a.loop_count; i0 += kBwdDepth<kMode>) {
 #pragma unroll
       for (int s = 0; s < kBwdDepth<kMode>; ++s) {
-        if (i0 + s < a.loop_count) {
-          const int64_t row = p + (int64_t)(i0 + s) * step;
-          uint4 q[kBwdStreams];
+        // unconditional turnover, as in bn_stats_partial_kernel
+        const int64_t row = p + (int64_t)(i0 + s) * step;
+        uint4 q[kBwdStreams];
 #pragma unroll
-          for (int t = 0; t < kBwdStreams; ++t) q[t] = buf[s][t];
-          load_bwd_row<kMode, kTwo>(a, v, row + kBwdDepth<kMode> * step, buf[s]);
+        for (int t = 0; t < kBwdStreams; ++t) q[t] = buf[s][t];
+        load_bwd_row<kMode, kTwo>(a, v, row + kBwdDepth<kMode> * step, buf[s]);
+        if (i0 + s < a.loop_count) {
           uint32_t dz_bits[4];
 #pragma unroll
           for (int k = 0; k < kVec; ++k) {
@@ -989,10 +1004,10 @@ extern "C" int tok_bn_stats_fwd(const void* x, int64_t rows, int channels, doubl
   a.momentum = (float)momentum;
   a.bessel = (float)((double)rows / (double)(rows - 1));
 
-  // the partial kernel: block (tile, block_y), one 8-channel vector per thread
-  int tile = kStatsPartialThreads / g.block_y;
+  // the partial kernel: block (4 * tile, block_y), one chain of an 8-channel vector per lane
+  int tile = kStatsPartialThreads / (kStatsChains * g.block_y);
   if (tile > a.vecs) tile = a.vecs;
-  const dim3 block(tile, g.block_y);
+  const dim3 block(kStatsChains * tile, g.block_y);
   const dim3 grid((a.vecs + tile - 1) / tile, g.grid_y);
   cudaStream_t st = (cudaStream_t)cuda_stream;
   bn_stats_partial_kernel<<<grid, block, 0, st>>>(a);
